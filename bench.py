@@ -7,13 +7,15 @@ random-init weights of the named shapes (no network for checkpoints).  One "step
 `EaModel.eagenerate(prompt, max_new_tokens=256)` call (prefill + decode cycles), as the reference times it
 (eagle/evaluation/gen_ea_answer_llama3chat.py:159-169).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]          # this repo's CUDA engine
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this repo's CUDA engine
     python bench.py --impl reference [...]                       # the reference algorithm (CPU oracle port) on host cores
 
 Prints ONE JSON line (rank 0).  `value` is measured with the prompt already resident in HBM; `e2e` goes through
 the public `EaModel.eagenerate` with a pinned-host prompt and host result (H2D/D2H inside the timed region).
-`roofline` is for the dominant kernel (the tcgen05/TMA skinny weight-streaming GEMM): algorithmic weight bytes of
+`roofline` is for the dominant kernel (the wgmma/TMA skinny weight-streaming GEMM): algorithmic weight bytes of
 its launches / their CUDA-event durations, measured in extra profiled steps right after the timed region.
+--dump-outputs DIR writes what the last timed step returned (generated ids, new-token and cycle counts) as DIR/<name>.npy
+(float64), so that two builds can be compared output for output: inputs and weights are seeded, identical from run to run.
 """
 from __future__ import annotations
 
@@ -72,24 +74,13 @@ def baseline_config(args) -> str:
     return b.get(args.tree, b["dynamic"])
 
 
-def profile_traffic_ratio():
-    """DRAM bytes / algorithmic bytes of the dominant kernel, measured with `ncu --set full` by tools/final_run.sh and stored in
-    profiles/ (dram__bytes_read.sum + dram__bytes_write.sum per launch over the weight bytes of that launch)."""
-    p = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return float(d["dram_over_algorithmic"]), d.get("source", p)
-    return None, "no ncu traffic capture committed for this kernel yet"
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -323,7 +314,7 @@ def cpu_reference_run(args, cycles: int, threads: int):
 
 
 def torch_cuda_reference_run(args, cycles: int):
-    """BASELINE.md 2's "practical bar": the reference ALGORITHM as eager PyTorch ops on the B200 itself (the oracle port with its
+    """BASELINE.md 2's "practical bar": the reference ALGORITHM as eager PyTorch ops on the GPU itself (the oracle port with its
     tensors on `cuda`; the reference proper cannot travel to the GPU box).  Same extrapolation as the CPU arm."""
     from oracle import eagle_oracle as orc
     from eagle_b200 import synthetic as syn
@@ -381,7 +372,7 @@ def run_reference_arm(args):
         print(json.dumps({"impl": "reference-eager-torch-on-cuda", "metric": "tokens/sec (bs=1)", "value": round(toks, 3), "unit": "tokens/s",
                           "tau": round(tau, 3), "dtype": args.dtype, "config": {"workload": workload_name(args)}, "detail": detail,
                           "what": "the CPU oracle port (reference algorithm, eager torch ops, HF-style dense masks, Python tree bookkeeping) with its "
-                                  "tensors on the B200; extrapolated to the 256-token job from measured prefill and per-cycle times"}), flush=True)
+                                  "tensors on the GPU; extrapolated to the 256-token job from measured prefill and per-cycle times"}), flush=True)
         return
     cores = min(effective_cores(), args.cpu_threads) if args.cpu_threads > 0 else effective_cores()
     cycles = max(2, args.steps + args.warmup)
@@ -466,23 +457,34 @@ def tp_parity_check(world: int, rank: int, device: int):
 
 
 def timed_steps(m, prompt, steps, dist, gen_kw):
-    """K eagenerate calls bracketed by barrier + synchronize, timed with CUDA events on the engine's stream."""
+    """K eagenerate calls bracketed by barrier + synchronize, timed with CUDA events on the engine's stream.
+    Also returns what the last call returned: (ids, new_token, idx)."""
     stream = m.cuda_stream()
     if dist is not None:
         dist.barrier()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(stream)
-    new_tokens, cycles = 0, 0
+    new_tokens, cycles, last = 0, 0, None
     for _ in range(steps):
-        _, nt, idx = m.eagenerate(prompt, max_new_tokens=NEW_TOKENS, max_length=2048, log=True, **gen_kw)
-        new_tokens += nt
-        cycles += idx + 1
+        last = m.eagenerate(prompt, max_new_tokens=NEW_TOKENS, max_length=2048, log=True, **gen_kw)
+        new_tokens += last[1]
+        cycles += last[2] + 1
     e1.record(stream)
     torch.cuda.synchronize()
     if dist is not None:
         dist.barrier()
-    return e0.elapsed_time(e1), new_tokens, cycles
+    return e0.elapsed_time(e1), new_tokens, cycles, last
+
+
+def dump_outputs(out_dir, last):
+    """The arrays the timed eagenerate call returned in its last step, as float64 .npy files (token ids are exact in float64)."""
+    import numpy as np
+    ids, new_token, idx = last
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "ids.npy"), ids.detach().cpu().to(torch.float64).numpy())
+    np.save(os.path.join(out_dir, "new_token.npy"), np.array([new_token], dtype=np.float64))
+    np.save(os.path.join(out_dir, "cycles.npy"), np.array([idx + 1], dtype=np.float64))
 
 
 def run_ours(args):
@@ -525,11 +527,13 @@ def run_ours(args):
     sampler = ClockSampler(local)
     sampler.start()
     log("timed region")
-    ms_dev, new_tokens, cycles = timed_steps(m, prompt_dev, args.steps, dist, gen_kw)   # inputs resident in HBM
+    ms_dev, new_tokens, cycles, last = timed_steps(m, prompt_dev, args.steps, dist, gen_kw)   # inputs resident in HBM
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     st = m.stats()
     launches = st["kernel_launches"]
     chain_stats = {k: st[k] for k in ("chain_ms", "chain_bytes", "chain_launches")}
-    ms_e2e, new_tokens_e, _ = timed_steps(m, prompt_host, args.steps, dist, gen_kw)     # pinned-host prompt, host result
+    ms_e2e, new_tokens_e, _, _ = timed_steps(m, prompt_host, args.steps, dist, gen_kw)     # pinned-host prompt, host result
     clocks = sampler.stop()
     if dist is not None:
         t = torch.tensor([ms_dev, ms_e2e], device="cuda")
@@ -569,15 +573,13 @@ def run_ours(args):
     ach = ps["gemm_bytes"] / 1e9 / (ps["gemm_ms"] / 1e3) if ps["gemm_ms"] > 0 else 0.0
     vach = ps["verify_gemm_bytes"] / 1e9 / (ps["verify_gemm_ms"] / 1e3) if ps["verify_gemm_ms"] > 0 else 0.0
     total_ms = ps["gemm_ms"] + ps["attn_ms"] + ps["other_ms"]
-    ratio, ratio_src = profile_traffic_ratio()
     chain = bool(os.environ.get("EB200_CHAIN", "") == "1")
-    roofline = {"kernel": ("gemm_chain_kernel (persistent per-layer chain: TMA + tcgen05.mma weight streaming, stream-K, fused RMSNorm / SwiGLU / RoPE / "
-                           "arg-max finishes) + skinny_gemm_tcgen05 (draft head), all launches") if chain else
-                          "skinny_gemm_tcgen05 (TMA + tcgen05.mma weight-streaming GEMM, cluster split-K; lm_head as a reduction-free chain launch "
+    roofline = {"kernel": ("gemm_chain_kernel (persistent per-layer chain: TMA + wgmma weight streaming, stream-K, fused RMSNorm / SwiGLU / RoPE / "
+                           "arg-max finishes) + skinny_gemm_wgmma (draft head), all launches") if chain else
+                          "skinny_gemm_wgmma (TMA + wgmma weight-streaming GEMM, cluster split-K; lm_head as a reduction-free chain launch "
                           "with fused arg-max), all launches",
                 "bound": "hbm", "achieved": round(ach, 1), "peak": peak, "unit": "GB/s", "frac": round(ach / peak, 4),
-                "traffic": round(ratio * ps["gemm_bytes"] / max(1, ps["gemm_launches"])) if ratio else None,
-                "traffic_source": ratio_src, "peak_source": peak_src, "launches": int(ps["gemm_launches"]),
+                "peak_source": peak_src, "launches": int(ps["gemm_launches"]),
                 "bytes_per_launch_avg": round(ps["gemm_bytes"] / max(1, ps["gemm_launches"])),
                 "us_per_launch_avg": round(1e3 * ps["gemm_ms"] / max(1, ps["gemm_launches"]), 2),
                 "verify_gemm": {"achieved": round(vach, 1), "frac": round(vach / peak, 4)},
@@ -643,7 +645,7 @@ def run_ours(args):
             except Exception as ex:
                 line["cpu_baseline"] = {"value": None, "unit": "tokens/s", "cores": effective_cores(), "kind": "port",
                                         "sample": f"CPU arm failed: {ex!r}"}
-            # BASELINE.md 2: the reference algorithm as eager PyTorch on this same B200 (extra key; own child process)
+            # BASELINE.md 2: the reference algorithm as eager PyTorch on this same GPU (extra key; own child process)
             try:
                 cmd2 = [sys.executable, os.path.abspath(__file__), "--impl", "reference", "--ref-device", "cuda", "--steps", "10", "--warmup", "2",
                         "--tree", args.tree, "--model", args.model, "--dtype", args.dtype]
@@ -651,9 +653,9 @@ def run_ours(args):
                     cmd2 += ["--layers", str(args.layers)]
                 out2 = subprocess.run(cmd2, capture_output=True, text=True, timeout=180, cwd=ROOT)
                 ref2 = json.loads([l for l in out2.stdout.splitlines() if l.startswith("{")][-1])
-                line["eager_torch_on_b200"] = {"value": ref2["value"], "unit": "tokens/s", "tau": ref2["tau"], "detail": ref2["detail"], "what": ref2["what"]}
+                line["eager_torch_on_gpu"] = {"value": ref2["value"], "unit": "tokens/s", "tau": ref2["tau"], "detail": ref2["detail"], "what": ref2["what"]}
             except Exception as ex:
-                line["eager_torch_on_b200"] = {"value": None, "error": repr(ex)[:300]}
+                line["eager_torch_on_gpu"] = {"value": None, "error": repr(ex)[:300]}
         print(json.dumps(line), flush=True)
     if dist is not None:
         dist.barrier()
@@ -675,12 +677,16 @@ def main():
                     help="random = random-init weights (tau = 1, the headline); correlated = bigram target + copy head at the same shapes (tau > 1)")
     ap.add_argument("--layers", type=int, default=0, help="override the number of target layers (debugging; 0 = the model's own)")
     ap.add_argument("--ref-device", default="cpu", choices=["cpu", "cuda"],
-                    help="--impl reference only: cpu = the driver's reference arm (host cores); cuda = the same port as eager PyTorch on the GPU")
+                    help="--impl reference only: cpu = the reference arm on host cores; cuda = the same port as eager PyTorch on the GPU")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-cycles", type=int, default=6)
     ap.add_argument("--cpu-threads", type=int, default=0, help="threads of the CPU arm (0 = all effective cores)")
     ap.add_argument("--cpu-timeout", type=int, default=240)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float64) for output-for-output comparisons")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.dtype is None:
         args.dtype = MODELS[args.model]["dtype"]
     if args.impl == "reference":

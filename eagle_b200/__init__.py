@@ -1,4 +1,4 @@
-"""eagle_b200: a B200-native (sm_100a) engine for EAGLE speculative decoding.
+"""eagle_b200: an H100-native (sm_90a) engine for EAGLE speculative decoding.
 
 `EaModel` keeps the reference's API (SafeAILab/EAGLE eagle/model/ea_model.py) and checkpoint
 format; the draft -> verify -> accept cycle runs in libeagle_b200.so (include/eagle_b200.h).

@@ -1,7 +1,7 @@
 """ctypes binding of libeagle_b200.so (C ABI declared in include/eagle_b200.h).
 
 There is no CPU path: importing this module on a box without the built library raises, and
-engine creation on a box without a B200 fails inside the library (eb200_create).
+engine creation on a machine without an H100 (sm_90) fails inside the library (eb200_create).
 """
 from __future__ import annotations
 

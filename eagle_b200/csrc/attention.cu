@@ -17,8 +17,8 @@
 // SWIZZLE_128B boxes per 64-row tile, completion on an mbarrier) issued by a dedicated producer warp; the eight consumer
 // warps release a slot through a second mbarrier, so there is no CTA-wide barrier per tile and the L2 latency of a tile is
 // hidden behind the previous tiles' MMAs.  Both matmuls run on the
-// tensor cores via mma.sync m16n8k16 + ldmatrix (the problem is ~1 GFLOP per layer and latency bound -- far below
-// where a TMEM round trip pays; the weight-streaming GEMMs are the tcgen05 kernels).
+// tensor cores via mma.sync m16n8k16 + ldmatrix (the problem is ~1 GFLOP per layer and latency bound; the weight-streaming
+// GEMMs are the wgmma kernels).
 #include <stdlib.h>
 
 #include "common.cuh"

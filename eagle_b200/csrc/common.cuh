@@ -1,6 +1,6 @@
-// Shared device helpers for the eagle_b200 kernels (sm_100a only).
+// Shared device helpers for the eagle_b200 kernels (sm_90a only).
 //   * dtype traits for the two model dtypes the reference runs in (bf16, fp16)
-//   * raw PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld)
+//   * raw PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors)
 // No CUTLASS/CuTe: everything the kernels need is spelled out here.
 #pragma once
 #include <cuda.h>
@@ -14,8 +14,8 @@
 
 #include <utility>
 
-#if defined(__CUDA_ARCH__) && !(defined(__CUDA_ARCH_FEAT_SM100_ALL) || defined(__CUDA_ARCH_FEAT_SM101_ALL))
-#error "eagle_b200 kernels are written for sm_100a (tcgen05 / TMEM / TMA)"
+#if defined(__CUDA_ARCH__) && !defined(__CUDA_ARCH_FEAT_SM90_ALL)
+#error "eagle_b200 kernels are written for sm_90a (wgmma / TMA / clusters)"
 #endif
 
 namespace eb {
@@ -27,14 +27,12 @@ template <typename T> struct DT;
 template <> struct DT<__nv_bfloat16> {
   using type = __nv_bfloat16;
   using type2 = __nv_bfloat162;
-  static constexpr int kUmmaFormat = 1;  // F16F32Format::BF16
   static __device__ __forceinline__ float to_f(type v) { return __bfloat162float(v); }
   static __device__ __forceinline__ type from_f(float v) { return __float2bfloat16_rn(v); }
 };
 template <> struct DT<__half> {
   using type = __half;
   using type2 = __half2;
-  static constexpr int kUmmaFormat = 0;  // F16F32Format::F16
   static __device__ __forceinline__ float to_f(type v) { return __half2float(v); }
   static __device__ __forceinline__ type from_f(float v) { return __float2half_rn(v); }
 };
@@ -97,6 +95,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// The same bounded wait without the printf, for the pipeline waits of kernels that issue wgmma: ptxas serialises every
+// wgmma of a kernel when a printf call may run while MMAs are in flight.
+__device__ __forceinline__ void mbar_wait_mma(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > (1u << 26)) __trap();
+  }
+}
 
 // ------------------------------------------------------------------------------------------
 // TMA
@@ -132,75 +138,123 @@ __device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUte
 }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (Hopper warpgroup MMA): D[64 x N] (fp32, registers of the 128 threads of one warpgroup) += A[64 x 16] * B[N x 16]^T,
+// A and B read from shared memory through matrix descriptors, both K-major.
 // ------------------------------------------------------------------------------------------
-template <int kCols> __device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: power of two in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads/writes across the asynchronous MMAs
+template <int R> __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-template <int kCols> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread on behalf of the CTA
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once every tcgen05.mma issued so far by this thread has completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// the same arrival on the barrier at this offset in every CTA of cta_mask (a slot shared through TMA multicast is free only when
-// every CTA that received it has consumed it)
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread (thread t <-> TMEM lane base+t)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-      " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // K-major, SWIZZLE_128B shared-memory matrix descriptor (tile rows of 64 x 2-byte elements = 128 B; 8-row
-// swizzle atoms of 1024 B).  Fields (SM100 UMMA SmemDescriptor): [0,14) start>>4, [16,30) LBO>>4 (unused for
-// swizzled K-major, set 1), [32,46) SBO>>4 (= 1024 B between 8-row groups), [46,48) version = 1,
-// [61,64) layout type = 2 (SWIZZLE_128B).
+// swizzle atoms of 1024 B; tiles 1024-B aligned).  Fields (sm_90 GMMA descriptor): [0,14) start>>4, [16,30) LBO>>4
+// (unused for swizzled K-major, set 1), [32,46) SBO>>4 (= 1024 B between 8-row groups), [49,52) base offset = 0,
+// [62,64) layout type = 1 (SWIZZLE_128B).  Advancing 16 K-elements (32 B) inside the swizzle row is +2 on the start field.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// kind::f16 instruction descriptor: fp32 accumulate, A and B K-major, M x N tile
-template <typename T> __host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4)                                      // c_format = F32
-         | (static_cast<uint32_t>(DT<T>::kUmmaFormat) << 7)   // a_format
-         | (static_cast<uint32_t>(DT<T>::kUmmaFormat) << 10)  // b_format
-         | (static_cast<uint32_t>(N >> 3) << 17)        // n_dim
-         | (static_cast<uint32_t>(M >> 4) << 24);       // m_dim
+
+// D (+)= A * B with scale-d = 1: callers zero the accumulators before the first MMA of a tile
+template <typename T, int N> struct Wgmma;
+template <> struct Wgmma<__nv_bfloat16, 16> {
+  static __device__ __forceinline__ void mma(float (&d)[8], uint64_t a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b));
+  }
+};
+template <> struct Wgmma<__half, 16> {
+  static __device__ __forceinline__ void mma(float (&d)[8], uint64_t a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b));
+  }
+};
+template <> struct Wgmma<__nv_bfloat16, 64> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b));
+  }
+};
+template <> struct Wgmma<__half, 64> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b));
+  }
+};
+template <> struct Wgmma<__nv_bfloat16, 256> {
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a), "l"(b));
+  }
+};
+template <> struct Wgmma<__half, 256> {
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a), "l"(b));
+  }
+};
+
+// One 64 x 16 K-block chunk of the tile: the four k16 steps of a 64-element (128-byte) K block
+template <typename T, int N>
+__device__ __forceinline__ void wgmma_kblock(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) Wgmma<T, N>::mma(d, a_desc + 2 * k, b_desc + 2 * k);
+}
+
+// Writes one warpgroup's m64nN fp32 accumulator fragment to shared memory as buf[n * ld + row0 + m] (m: the 64 rows of the
+// warpgroup's A operand, n: the N columns), the column-major [N][128] tile layout the epilogues read (thread <-> row).
+// Fragment layout: thread t (warp w = t / 32, lane l) holds, for each 8-column block i, rows 16w + l/4 (+8) and
+// columns 8i + 2(l%4) (+1).
+template <int N>
+__device__ __forceinline__ void wgmma_store_acc(const float (&d)[N / 2], float* buf, int ld, int row0) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2);
+  const int c = 2 * (t & 3);
+  const uint32_t base = smem_u32(buf);
+  auto st = [&](int col, int row, float v) {
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(base + static_cast<uint32_t>((col * ld + row) * 4)), "f"(v) : "memory");
+  };
+#pragma unroll
+  for (int i = 0; i < N / 8; ++i) {
+    st(8 * i + c, r, d[4 * i + 0]);
+    st(8 * i + c + 1, r, d[4 * i + 1]);
+    st(8 * i + c, r + 8, d[4 * i + 2]);
+    st(8 * i + c + 1, r + 8, d[4 * i + 3]);
+  }
+}
+
+// the 16 fp32 columns [c0, c0 + 16) of accumulator row `row` of a [N][ld] shared-memory tile (see wgmma_store_acc)
+__device__ __forceinline__ void acc_ld16(const float* buf, int ld, int row, int c0, float (&r)[16]) {
+  const uint32_t base = smem_u32(buf) + static_cast<uint32_t>((c0 * ld + row) * 4);
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(r[j]) : "r"(base + static_cast<uint32_t>(j * ld * 4)) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -238,6 +292,10 @@ __device__ __forceinline__ float dsmem_ld_f32(uint32_t cluster_addr) {
   float v;
   asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(cluster_addr) : "memory");
   return v;
+}
+// arrive on the mbarrier at the offset of `bar` in the CTA of rank `rank` of this cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(dsmem_map(smem_u32(bar), rank)) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------

@@ -280,7 +280,7 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
   {
     int n_dev = 0;
     if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0)
-      return fail("no CUDA device visible: eagle_b200 has no CPU path (the engine is sm_100a CUDA only)");
+      return fail("no CUDA device visible: eagle_b200 has no CPU path (the engine is sm_90a CUDA only)");
   }
   if (c.dtype != EB200_BF16 && c.dtype != EB200_FP16) return fail("dtype must be bf16 or fp16");
   if (c.vocab_size < 1 || c.hidden_size < 128 || c.intermediate_size < 64 || c.num_layers < 1 || c.num_heads < 1 ||
@@ -306,7 +306,8 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
   CK(cudaSetDevice(c.device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, c.device));
-  if (prop.major != 10) return fail("device %d is sm_%d%d; eagle_b200 kernels are sm_100a only", c.device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail("device %d is sm_%d%d; eagle_b200 kernels are sm_90a (H100) only", c.device, prop.major, prop.minor);
 
   eb200_engine* e = new eb200_engine();
   e->c = c;
@@ -339,7 +340,7 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
   e->D = c.depth + 2;
   e->cap = c.max_length + 64;
   {
-    const char* pe = getenv("EB200_PREFILL_ROWS");  // 64 = round-1 behaviour (weights streamed once per 64 prompt tokens)
+    const char* pe = getenv("EB200_PREFILL_ROWS");  // 64 = weights streamed once per 64 prompt tokens instead of 256
     const int want = pe ? atoi(pe) : 256;
     e->act_rows = (want >= 256 && c.tp_size == 1 && !(c.flags & EB200_FLAG_SIMT_GEMM)) ? 256 : 64;
   }
@@ -820,12 +821,11 @@ extern "C" int eb200_finalize(eb200_engine* e) {
     if (e->d2t && !e->d2t_loaded) return fail("head d2t missing (draft_vocab_size != vocab_size)");
   }
   {
-    // Persistent chain launches (mega.cu).  Measured on one B200 (profiles/r02_chain_*): the layer segment as ONE launch is
-    // SLOWER than round 1's per-projection cluster split-K kernels (141 vs ~115 us per layer: its global-memory split-K
-    // reduction is bounded by the LSU path of the finishing SMs), so on one GPU only the lm_head runs as a (single-phase,
-    // reduction-free) chain launch with the fused arg-max (same speed as gemm + arg-max kernel, no 15 MB logits round trip).
-    // Under tensor parallelism the chain segment was measured slower as well (128.8 vs 167 tok/s at TP = 2), so the peer-window
-    // exchange runs as its own kernel behind the per-projection GEMMs (tp_fused.cu) and the chain segment stays opt-in.
+    // Persistent chain launches (mega.cu).  The layer segment as ONE launch is slower than the per-projection cluster split-K
+    // kernels (its global-memory split-K reduction is bounded by the LSU path of the finishing SMs), so on one GPU only the
+    // lm_head runs as a (single-phase, reduction-free) chain launch with the fused arg-max (no 15 MB logits round trip).
+    // Under tensor parallelism the chain segment is slower as well, so the peer-window exchange runs as its own kernel behind
+    // the per-projection GEMMs (tp_fused.cu) and the chain segment stays opt-in.
     //   EB200_CHAIN=0 : never;  EB200_CHAIN=1 : layer segments as chain launches (A/B);  EB200_CHAIN_DRAFT=1 : draft head tail too
     const char* env = getenv("EB200_CHAIN");
     const int mode = env ? atoi(env) : -1;  // -1 = default policy
@@ -940,9 +940,8 @@ static void debug_scan(eb200_engine* e, const char* label) {
 }
 
 // split-K factor (== cluster size) of the cluster GEMM: the smallest power of two that gives the launch >= ~100 CTAs
-// (one per SM on most SMs) with >= 4 k-blocks each.  Measured on the Llama-3-8B shapes (tools/gemm_bench.py, tools/sweep.sh):
-// odd cluster sizes schedule badly (qkv: 30.8 us at 3 vs 16.9 us at 4), and grids above 148 CTAs are individually as fast
-// but overlap worse with their PDL neighbours inside the cycle (6.76 ms/cycle at target 148 vs 6.37 ms at 100).
+// (one per SM on most SMs) with >= 4 k-blocks each.  Powers of two only: odd cluster sizes schedule badly, and a grid a
+// little below the SM count leaves room for the next kernel's programmatic-dependent-launch prologue.
 static int pick_splitk(int N, int K, int mpad, int epi, size_t ws_bytes) {
   (void)mpad; (void)epi; (void)ws_bytes;
   static int forced = -1, target = 0;
@@ -1235,7 +1234,7 @@ static int attention(eb200_engine* e, const RowCtx& cx, const void* q, void* kc,
     static long budget = -1;
     if (budget < 0) {
       const char* s = getenv("EB200_ATTN_PREFETCH_MB");
-      budget = (s ? atol(s) : 0) << 20;  // off by default: no measured gain (profiles/r02_chain_prefetch_ab.txt)
+      budget = (s ? atol(s) : 0) << 20;  // off by default (an experiment knob)
     }
     long left = budget;
     const Linear* nx[2] = {next0, next1};
@@ -1547,7 +1546,7 @@ static int target_segment_chain(eb200_engine* e, const RowCtx& cx, int i, void* 
 }
 
 // lm_head over the rows in e->xn (ea_model.py:190): one reduction-free chain launch (whole 128-row vocabulary tiles per CTA,
-// per-row arg-max straight from TMEM, merged per row) or, for the sampling path, the logits of this rank's shard.
+// per-row arg-max straight from the staged accumulator tile, merged per row) or, for the sampling path, the logits of this rank's shard.
 static int target_head(eb200_engine* e, const RowCtx& cx, int head_mode) {
   if (head_mode == HEAD_NONE) return 0;
   if (!e->chain_head) {
@@ -1901,7 +1900,7 @@ static int target_prefill(eb200_engine* e, const int64_t* prompt, int P, int* fi
   CK(cudaMemcpyAsync(e->ids_dev, prompt, static_cast<size_t>(P) * 8, cudaMemcpyDefault, e->stream));
   CK(cudaMemcpyAsync(e->out_ids_dev, e->ids_dev, static_cast<size_t>(P) * 8, cudaMemcpyDeviceToDevice, e->stream));
   int last_rows = 0;
-  // 256 prompt rows per pass where the activation buffers allow it (one GPU, tcgen05 path): the weights are streamed
+  // 256 prompt rows per pass where the activation buffers allow it (one GPU, wgmma path): the weights are streamed
   // ceil(P / 256) times instead of ceil(P / 64) times (utils.py:232-254 runs the whole prompt in one forward)
   const int chunk = (e->act_rows >= 256 && !e->chain_target) ? 256 : 64;
   for (int base = 0; base < P; base += chunk) {

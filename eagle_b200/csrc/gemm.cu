@@ -1,16 +1,16 @@
-// Skinny-M weight-streaming GEMM for sm_100a:  Y[m, n] = sum_k X[m, k] * W[n, k],  m <= MPAD in {16, 64}.
+// Skinny-M weight-streaming GEMM for sm_90a:  Y[m, n] = sum_k X[m, k] * W[n, k],  m <= MPAD in {16, 64, 256}.
 //
 // This is the dominant kernel of the draft -> verify -> accept cycle: at batch 1 every projection of the target
 // verify pass (60 tree rows) and of the draft head (10 rows) is HBM-bound on its weight matrix, so the job of the
 // kernel is to stream W once at HBM speed and keep the tensor pipe off the critical path.
 //
-//   * swap-AB: the 128 weight rows of a tile are the UMMA M dimension, the (padded) activation rows are UMMA N,
-//     so a tile is one tcgen05.mma.cta_group::1.kind::f16 of shape 128 x MPAD x 16 per 32 bytes of K.
+//   * swap-AB: the 128 weight rows of a tile are the wgmma M dimension, the (padded) activation rows are wgmma N,
+//     so a tile is two wgmma.m64nMPADk16 (one per MMA warpgroup) per 32 bytes of K.
 //   * W and X tiles (64 K-elements = 128 B rows, SWIZZLE_128B) are staged by TMA into a multi-stage shared-memory
 //     ring (mbarrier full/empty pairs); weights carry an L2 evict-first hint, activations evict-last.
-//   * one producer lane (warp 0) issues TMA, one MMA lane (warp 1) issues tcgen05.mma and tcgen05.commit, four
-//     epilogue warps read the fp32 accumulator from TMEM with tcgen05.ld (thread <-> weight row), 16 columns at a time.
-//   * split-K fills the 148 SMs for the small-N projections.  The CTAs that share an n-tile form a thread-block
+//   * one producer lane (warp 8) issues TMA, two MMA warpgroups (warps 0..7) issue wgmma and hold the fp32 accumulators in
+//     registers; at the end they park them in shared memory and warpgroup 0 runs the epilogue (thread <-> weight row).
+//   * split-K fills the SMs for the small-N projections.  The CTAs that share an n-tile form a thread-block
 //     CLUSTER (1 x splitk x 1): each parks its fp32 partial tile in its own shared memory, and after a cluster
 //     barrier every CTA reduces a slice of the activation rows over all peers through distributed shared memory
 //     (mapa + ld.shared::cluster) in fixed rank order -- deterministic, no global-memory workspace, no serial tail.
@@ -38,10 +38,10 @@ static int env_kb(const char* name, int dflt) {
 static int smem_budget(int total_ctas) {
   static int small_kb = 0, big_kb = 0;
   if (!small_kb) {
-    small_kb = env_kb("EB200_GEMM_SMEM_KB", 100);      // when > 148 CTAs (two per SM)
-    big_kb = env_kb("EB200_GEMM_SMEM_BIG_KB", 200);    // when <= 148 CTAs (one per SM)
+    small_kb = env_kb("EB200_GEMM_SMEM_KB", 100);      // when the grid exceeds the SM count (two per SM)
+    big_kb = env_kb("EB200_GEMM_SMEM_BIG_KB", 200);    // when it fits one CTA per SM
   }
-  return (total_ctas <= 148 ? big_kb : small_kb) * 1024;
+  return (total_ctas <= device_sm_count() ? big_kb : small_kb) * 1024;
 }
 static int stage_count_for(int mpad, int epi, int total_ctas) {
   // 256 activation rows (prefill): a stage is 48 KB and the cluster reduction parks 128 KB of partials, so always one CTA per SM
@@ -54,28 +54,29 @@ static int stage_count_for(int mpad, int epi, int total_ctas) {
 int gemm_stage_count(int mpad, int epi) { return stage_count_for(mpad, epi, 1 << 30); }
 
 // ------------------------------------------------------------------------------------------------------------
-// tcgen05 + TMA kernel
+// wgmma + TMA kernel
 // ------------------------------------------------------------------------------------------------------------
+// Warps 0..7 are two MMA warpgroups: warpgroup g multiplies weight rows [64g, 64g + 64) of the tile with the X tile
+// (wgmma m64 x MPAD x k16, fp32 accumulators in registers); warp 8 is the TMA producer.  After the main loop both
+// warpgroups park their accumulators in the (then idle) stage memory as an fp32 [acc][MPAD][128] tile, and warpgroup 0
+// runs the epilogue from there (thread <-> weight row).
 // XMC: the two CTAs of neighbouring n-tiles (cluster dimension x = 2) stream the SAME activation k-range; each loads one half of
-// every X tile (32 rows) and TMA-multicasts it into both CTAs' rings, so the L2 -> shared-memory ingress of an SM -- the
-// measured limiter of the 60-row projections (X is one third of every stage, DESIGN.md 6) -- carries half the X bytes.
+// every X tile (32 rows) and TMA-multicasts it into both CTAs' rings, so the L2 -> shared-memory ingress of an SM carries half
+// the X bytes.
 template <typename T, int MPAD, int EPI, bool XMC>
-__global__ void __launch_bounds__(kGemmThreads, 2)
-skinny_gemm_tcgen05(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmW2,
-                    const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXh, const GemmParams p, const int stages) {
+__global__ void __launch_bounds__(kGemmThreads, (MPAD >= 256 ? 1 : 2))
+skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmW2,
+                  const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXh, const GemmParams p, const int stages) {
   constexpr bool kDual = (EPI == EPI_SWIGLU);
   static_assert(!XMC || (MPAD == 64 && !kDual), "X multicast: 64-row tiles, single accumulator");
   constexpr int kStageBytes = stage_bytes(MPAD, EPI);
-  constexpr int kTmemCols = tmem_cols(MPAD, EPI);
-  constexpr uint32_t kIdesc = make_idesc_f16<T>(kBlockN, MPAD);
+  constexpr int kPartBytes = acc_tile_bytes(MPAD, EPI);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* ctrl = smem + stages * kStageBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);
   uint64_t* empty_bar = full_bar + kMaxStages;
-  uint64_t* tmem_full = empty_bar + kMaxStages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -96,19 +97,15 @@ skinny_gemm_tcgen05(const __grid_constant__ CUtensorMap tmW, const __grid_consta
     if (kDual) tma_prefetch_desc(&tmW2);
     for (int i = 0; i < stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], XMC ? 2 : 1);  // XMC: this CTA's MMAs and the neighbour's (its half of the X tile lives here too)
+      // one arrival per MMA warpgroup; XMC: also the neighbour's (its half of the X tile lives here too)
+      mbar_init(&empty_bar[i], XMC ? 4 : 2);
     }
-    mbar_init(tmem_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<kTmemCols>(tmem_ptr);
-  tc_fence_before();
   if (XMC) cluster_sync_all();  // the neighbour's barriers exist before anything is multicast into this CTA
   else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == kTmaWarp) {
     // ===== TMA producer =====
     if (lane == 0) {
       // The weight tiles do not depend on any earlier kernel: fill the whole ring with W before the programmatic
@@ -136,7 +133,7 @@ skinny_gemm_tcgen05(const __grid_constant__ CUtensorMap tmW, const __grid_consta
       int s = (pre == stages) ? 0 : pre;
       uint32_t ph = (pre == stages) ? 1 : 0;
       for (int kb = kb_begin + pre; kb < kb_end; ++kb) {
-        mbar_wait(&empty_bar[s], ph ^ 1);
+        mbar_wait_mma(&empty_bar[s], ph ^ 1);
         uint8_t* st = smem + s * kStageBytes;
         mbar_arrive_expect_tx(&full_bar[s], kStageBytes);
         tma_load_2d(st, &tmW, &full_bar[s], kb * kBlockK, n_tile * kBlockN, kEvictFirst);
@@ -148,81 +145,61 @@ skinny_gemm_tcgen05(const __grid_constant__ CUtensorMap tmW, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb) {
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + s * kStageBytes);
-        const uint32_t b_addr = a_addr + kWTileBytes * (kDual ? 2 : 1);
-        const uint64_t a_desc = make_kmajor_sw128_desc(a_addr);
-        const uint64_t b_desc = make_kmajor_sw128_desc(b_addr);
-        const uint32_t first = (kb == kb_begin) ? 0u : 1u;
-#pragma unroll
-        for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-          // advance 16 elements = 32 bytes inside the 128-byte swizzle row: +2 in the (addr >> 4) field
-          umma_f16(tmem_base, a_desc + 2 * k, b_desc + 2 * k, kIdesc, (k > 0) ? 1u : first);
-        }
-        if (kDual) {
-          const uint64_t a2_desc = make_kmajor_sw128_desc(a_addr + kWTileBytes);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k)
-            umma_f16(tmem_base + MPAD, a2_desc + 2 * k, b_desc + 2 * k, kIdesc, (k > 0) ? 1u : first);
-        }
-        if constexpr (XMC) umma_commit_multicast(&empty_bar[s], pair_mask);  // frees the slot here AND tells the neighbour this half is consumed
-        else umma_commit(&empty_bar[s]);  // frees the smem slot once these MMAs retire
-        if (++s == stages) {
-          s = 0;
-          ph ^= 1;
-        }
-      }
-      umma_commit(tmem_full);
-    }
   } else {
-    // ===== epilogue warps (TMEM lane quadrant = warp % 4) =====
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    pdl_wait();  // residual / device state / KV cache are produced by earlier kernels
-    const int m_valid = valid_rows(p);
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    // every TMA load has landed and every MMA has retired: stage memory is free scratch for the epilogue
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16);
-    auto load_chunk = [&](int c, float(&acc)[16], float(&acc2)[16]) {
-      uint32_t r[16];
-      tmem_ld16(taddr + c * 16, r);
-      tmem_ld_wait();
+    // ===== MMA warpgroups =====
+    const int wg = warp >> 2;
+    float acc[MPAD / 2], acc2[kDual ? MPAD / 2 : 1];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) acc[j] = __uint_as_float(r[j]);
-      if constexpr (kDual) {
-        tmem_ld16(taddr + MPAD + c * 16, r);
-        tmem_ld_wait();
+    for (int i = 0; i < MPAD / 2; ++i) acc[i] = 0.f;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) acc2[j] = __uint_as_float(r[j]);
+    for (int i = 0; i < (kDual ? MPAD / 2 : 1); ++i) acc2[i] = 0.f;
+    auto release = [&](int st) {
+      if ((threadIdx.x & 127) == 0) {
+        mbar_arrive(&empty_bar[st]);
+        if constexpr (XMC) mbar_arrive_cluster(&empty_bar[st], crank ^ 1u);  // the neighbour's half of this slot is consumed too
       }
     };
-    float acc[16], acc2[16];
-    if (p.splitk == 1) {
-#pragma unroll 1
-      for (int c = 0; c < MPAD / 16; ++c) {
-        if (c * 16 >= m_valid) break;
-        load_chunk(c, acc, acc2);
-        final_chunk<T, EPI>(p, acc, acc2, c * 16, m_valid, row, n_tile, smem);
+    int s = 0, prev = -1;
+    uint32_t ph = 0;
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+      mbar_wait_mma(&full_bar[s], ph);
+      const uint32_t st = smem_u32(smem + s * kStageBytes);
+      const uint32_t a_addr = st + wg * (kWTileBytes / 2);  // 64 weight rows = 8 KB = eight whole swizzle atoms
+      const uint64_t b_desc = make_kmajor_sw128_desc(st + kWTileBytes * (kDual ? 2 : 1));
+      wgmma_fence();
+      wgmma_kblock<T, MPAD>(acc, make_kmajor_sw128_desc(a_addr), b_desc);
+      if constexpr (kDual) wgmma_kblock<T, MPAD>(acc2, make_kmajor_sw128_desc(a_addr + kWTileBytes), b_desc);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's MMAs have retired: its slot can be refilled
+      if (prev >= 0) release(prev);
+      prev = s;
+      if (++s == stages) {
+        s = 0;
+        ph ^= 1;
       }
-    } else {
-      // park the fp32 partial tile in this CTA's shared memory: part[acc][m][128]
-      float* part = reinterpret_cast<float*>(smem);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    wgmma_fence_acc(acc2);
+    // every MMA of both warpgroups has retired and every TMA load has landed: the stage memory becomes the fp32
+    // accumulator tile part[acc][m][128], then scratch for the epilogue
+    asm volatile("bar.sync 2, 256;" ::: "memory");
+    float* part = reinterpret_cast<float*>(smem);
+    wgmma_store_acc<MPAD>(acc, part, kBlockN, wg * 64);
+    if constexpr (kDual) wgmma_store_acc<MPAD>(acc2, part + MPAD * kBlockN, kBlockN, wg * 64);
+    asm volatile("bar.sync 2, 256;" ::: "memory");
+    if (wg == 0) {
+      pdl_wait();  // residual / device state / KV cache are produced by earlier kernels
+      if (p.splitk == 1) {
+        const int row = threadIdx.x;
+        const int m_valid = valid_rows(p);
+        float a[16], a2[16];
 #pragma unroll 1
-      for (int c = 0; c < MPAD / 16; ++c) {
-        if (c * 16 >= m_valid) break;
-        load_chunk(c, acc, acc2);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          part[(c * 16 + j) * kBlockN + row] = acc[j];
-          if constexpr (kDual) part[(MPAD + c * 16 + j) * kBlockN + row] = acc2[j];
+        for (int c = 0; c < MPAD / 16; ++c) {
+          if (c * 16 >= m_valid) break;
+          acc_ld16(part, kBlockN, row, c * 16, a);
+          if constexpr (kDual) acc_ld16(part + MPAD * kBlockN, kBlockN, row, c * 16, a2);
+          final_chunk<T, EPI>(p, a, a2, c * 16, m_valid, row, n_tile, smem + kPartBytes);
         }
       }
     }
@@ -231,16 +208,14 @@ skinny_gemm_tcgen05(const __grid_constant__ CUtensorMap tmW, const __grid_consta
   if (p.splitk > 1) {
     // ===== cluster split-K reduction over distributed shared memory =====
     cluster_sync_all();  // every peer's partial tile is visible cluster-wide
-    if (warp >= 2) {
-      const int quad = warp & 3;
-      const int row = quad * 32 + lane;
+    if (warp < 4) {
+      const int row = threadIdx.x;
       const int m_valid = valid_rows(p);
       const int S = p.splitk;
       const int rank = static_cast<int>(XMC ? (crank >> 1) : crank);  // this CTA's index among the split-K peers of its n-tile
       const int per = (MPAD + S - 1) / S;  // activation rows reduced by each CTA
       const int m_lo = rank * per, m_hi = min(MPAD, m_lo + per);
       const uint32_t part_local = smem_u32(smem);
-      constexpr int kPartBytes = (kDual ? 2 : 1) * MPAD * kBlockN * 4;
       float acc[16], acc2[16];
 #pragma unroll 1
       for (int m0 = m_lo; m0 < m_hi; m0 += 16) {
@@ -265,10 +240,6 @@ skinny_gemm_tcgen05(const __grid_constant__ CUtensorMap tmW, const __grid_consta
   } else if (XMC) {
     cluster_sync_all();  // the neighbour may still multicast into / arrive on this CTA's shared memory
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<kTmemCols>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -364,8 +335,8 @@ const void* silu_lut(int dtype, cudaStream_t s) {
 static bool xmc_enabled() {
   static int v = -1;
   if (v < 0) {
-    // Measured (profiles/r02_gemm_xmulticast_ab.txt): correct (all GEMM parity tests pass with it) but not faster -- gate/up 43.3 vs
-    // 43.2 us with pairs, and the (2, 4, 1) clusters of the split-K projections schedule badly (o_proj 33 vs 18 us) -- so opt-in.
+    // Opt-in: correct (all GEMM parity tests pass with it), but it doubles the cluster size of the split-K projections, which
+    // constrains their scheduling, and has no measured gain on the H100.
     const char* e = getenv("EB200_GEMM_XMC");
     v = (e && atoi(e) == 1) ? 1 : 0;
   }
@@ -386,13 +357,13 @@ static int launch_one(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUt
 template <typename T, int MPAD, int EPI, bool XMC>
 static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
                         cudaStream_t s) {
-  auto kern = skinny_gemm_tcgen05<T, MPAD, EPI, XMC>;
+  auto kern = skinny_gemm_wgmma<T, MPAD, EPI, XMC>;
   dim3 grid((p.N + kBlockN - 1) / kBlockN, p.splitk);
   const int stages = stage_count_for(MPAD, EPI, static_cast<int>(grid.x * grid.y));
   const int smem = stages * stage_bytes(MPAD, EPI) + kCtrlBytes + 1024;
   if (p.splitk > 8) return static_cast<int>(cudaErrorInvalidValue);  // portable cluster size
-  // the cluster reduction parks (1|2) x MPAD x 128 fp32 partials (+ a 4 KB exchange strip) in the stage memory
-  if (p.splitk > 1 && stages * stage_bytes(MPAD, EPI) < (EPI == EPI_SWIGLU ? 2 : 1) * MPAD * kBlockN * 4 + 4096)
+  // the accumulators are parked as (1|2) x MPAD x 128 fp32 partials (+ a 4 KB exchange strip) in the stage memory
+  if (stages * stage_bytes(MPAD, EPI) < acc_tile_bytes(MPAD, EPI) + 4096)
     return static_cast<int>(cudaErrorInvalidValue);
   static bool configured_dev[64] = {};  // per device (the attribute is per device) and per instantiation
   const int cur_dev = current_device_index();
@@ -420,7 +391,7 @@ static int launch_epi(int epi, const CUtensorMap* a, const CUtensorMap* b, const
   return static_cast<int>(cudaErrorInvalidValue);
 }
 
-// 256 activation rows per launch (prompt prefill: UMMA N = 256, the weights are streamed once per 256 prompt tokens instead of
+// 256 activation rows per launch (prompt prefill: wgmma N = 256, the weights are streamed once per 256 prompt tokens instead of
 // once per 64): only the epilogues the target's decoder layer needs
 template <typename T>
 static int launch_epi256(int epi, const CUtensorMap* a, const CUtensorMap* c, const GemmParams& p, cudaStream_t s) {

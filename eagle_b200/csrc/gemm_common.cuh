@@ -1,4 +1,4 @@
-// Tile constants and the epilogue device functions shared by the two tcgen05 GEMM kernels (cluster split-K in gemm.cu,
+// Tile constants and the epilogue device functions shared by the two wgmma GEMM kernels (cluster split-K in gemm.cu,
 // persistent stream-K in gemm_streamk.cu) and the SIMT bring-up kernel.
 #pragma once
 #include "common.cuh"
@@ -6,10 +6,10 @@
 
 namespace eb {
 
-constexpr int kBlockN = 128;  // weight rows per tile == UMMA M
+constexpr int kBlockN = 128;  // weight rows per tile == two wgmma M = 64 halves
 constexpr int kBlockK = 64;   // K elements per stage == one 128-byte swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kGemmThreads = 192;  // warp0 TMA, warp1 MMA + TMEM alloc, warps 2..5 epilogue
+constexpr int kGemmThreads = 288;  // warps 0..7: two MMA warpgroups (gemm.cu) or MMA + epilogue warpgroups (stream-K); warp 8 TMA
+constexpr int kTmaWarp = 8;
 constexpr int kWTileBytes = kBlockN * kBlockK * 2;
 constexpr int kMaxStages = 12;
 constexpr int kCtrlBytes = 1024;
@@ -18,9 +18,20 @@ __host__ __device__ constexpr int x_tile_bytes(int mpad) { return mpad * kBlockK
 __host__ __device__ constexpr int stage_bytes(int mpad, int epi) {
   return kWTileBytes * (epi == EPI_SWIGLU ? 2 : 1) + x_tile_bytes(mpad);
 }
-__host__ __device__ constexpr int tmem_cols(int mpad, int epi) {
-  int c = mpad * (epi == EPI_SWIGLU ? 2 : 1);
-  return c <= 32 ? 32 : (c <= 64 ? 64 : (c <= 128 ? 128 : 256));
+// fp32 accumulator tile(s) of one CTA staged in shared memory: [acc][MPAD][128]
+__host__ __device__ constexpr int acc_tile_bytes(int mpad, int epi) { return (epi == EPI_SWIGLU ? 2 : 1) * mpad * kBlockN * 4; }
+
+// number of SMs of the current device (the grids are sized to fill it)
+inline int device_sm_count() {
+  static int n[64] = {};
+  const int dev = current_device_index();
+  if (dev < 0) return 1;
+  if (!n[dev]) {
+    int v = 0;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v < 1) v = 1;
+    n[dev] = v;
+  }
+  return n[dev];
 }
 
 // T(silu(g)) of an already-rounded g through the 64K-entry table (kernels.h: silu_lut)
@@ -34,7 +45,7 @@ __device__ __forceinline__ int dyn(const int* st, DynInt d) { return (d.idx >= 0
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------------------
-// Epilogue pieces shared by the tcgen05 kernel and the SIMT bring-up kernel.  They are called by exactly 128
+// Epilogue pieces shared by the wgmma kernels and the SIMT bring-up kernel.  They are called by exactly 128
 // threads; thread `row` (0..127) owns weight row n = n_tile*128 + row and processes the activation rows in
 // chunks of 16:  acc[j] is the fp32 accumulator of activation row m0 + j  (acc2: the `up` tile for SwiGLU).
 // ------------------------------------------------------------------------------------------------------------

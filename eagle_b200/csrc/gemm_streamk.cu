@@ -1,19 +1,20 @@
 // Persistent stream-K variant of the skinny weight-streaming GEMM (same math, tiles, epilogues and rounding points as
-// gemm.cu; see there for the swap-AB / TMA / tcgen05 layout).
+// gemm.cu; see there for the swap-AB / TMA / wgmma layout).
 //
-// Why: measured on B200 (tools/gemm_bench.py), one SM streams at most ~50 GB/s through this TMA pattern, so the HBM
-// roofline (6.5 TB/s) is only reachable when ALL 148 SMs stream, evenly, for the whole kernel.  Tile-granular grids
+// Why: the HBM roofline is only reachable when ALL SMs stream, evenly, for the whole kernel.  Tile-granular grids
 // (48 / 32 / 112 tiles for the Llama-3-8B projections, times a power-of-two split) leave SMs idle or double-loaded.
 // Here the iteration space  units = n_tiles x k_blocks  is cut into one contiguous, equal share per CTA (one CTA per
-// SM, <= 148 CTAs).  A CTA walks its share k-fastest; every change of tile closes a SEGMENT:
+// SM).  A CTA walks its share k-fastest; every change of tile closes a SEGMENT:
 //   * a segment that covers a whole tile runs the fused epilogue directly;
 //   * a segment that starts inside a tile (k > 0) is a CONTRIBUTION: its fp32 partial goes to a per-CTA slot of an
 //     L2-resident workspace, then the tile's arrival counter is bumped (release);
 //   * the segment that starts a tile (k == 0) but does not finish it makes this CTA the tile's FINISHER: it waits
 //     for the contributions (they come from the next CTAs, which process them FIRST, so the wait is short and can
 //     never deadlock: contributors never wait), adds them in CTA order (deterministic) and runs the epilogue.
-// The TMA producer streams across segment boundaries without draining, and the accumulator is double-buffered in
-// TMEM, so the MMAs of the next segment overlap the epilogue of the previous one.  Weight tiles are prefetched
+// Roles: warps 0..3 are the MMA warpgroup (wgmma, both 64-row halves of the tile, fp32 accumulators in registers), warps
+// 4..7 the epilogue, warp 8 the TMA producer.  The TMA producer streams across segment boundaries without draining; at
+// the end of a segment the MMA warpgroup hands its accumulators to the epilogue through a shared-memory staging tile and
+// goes on with the next segment, so the MMAs of the next segment overlap the epilogue of the previous one.  Weight tiles are prefetched
 // before the programmatic-dependent-launch wait (they do not depend on the previous kernel), activations after it.
 #include <stdio.h>
 #include <stdlib.h>
@@ -50,19 +51,16 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
   constexpr bool kDual = (EPI == EPI_SWIGLU);
   constexpr int kAcc = kDual ? 2 : 1;
   constexpr int kStageBytes = stage_bytes(MPAD, EPI);
-  constexpr int kBufCols = MPAD * kAcc;                  // TMEM columns of one accumulator buffer
-  constexpr int kTmemCols = (2 * kBufCols <= 32) ? 32 : (2 * kBufCols <= 64 ? 64 : (2 * kBufCols <= 128 ? 128 : 256));
-  constexpr uint32_t kIdesc = make_idesc_f16<T>(kBlockN, MPAD);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* scratch = smem + stages * kStageBytes;        // epilogue exchange strip (never aliased with the ring)
+  float* accbuf = reinterpret_cast<float*>(smem + stages * kStageBytes);  // [acc][MPAD][128] staged accumulators
+  uint8_t* scratch = smem + stages * kStageBytes + acc_tile_bytes(MPAD, EPI);  // epilogue exchange strip (never aliased with the ring)
   uint8_t* ctrl = scratch + kSkEpiScratch;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>((reinterpret_cast<uintptr_t>(ctrl) + 7) & ~static_cast<uintptr_t>(7));
   uint64_t* empty_bar = full_bar + kMaxStages;
-  uint64_t* tmem_full = empty_bar + kMaxStages;          // [2]
-  uint64_t* tmem_empty = tmem_full + 2;                  // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* acc_full = empty_bar + kMaxStages;   // the staging tile holds a segment's accumulators (128 arrivals)
+  uint64_t* acc_empty = acc_full + 1;            // the epilogue has drained it
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -78,19 +76,13 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 1);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 1);
-    }
+    mbar_init(acc_full, 128);
+    mbar_init(acc_empty, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<kTmemCols>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == kTmaWarp) {
     // ===== TMA producer: one contiguous stream of units, oblivious to segment boundaries =====
     if (lane == 0) {
       const long n_units = u1 - u0;
@@ -112,7 +104,7 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
       uint32_t ph = (pre == stages) ? 1 : 0;
       for (long u = u0 + pre; u < u1; ++u) {
         const int tile = static_cast<int>(u / sk.num_kb), kb = static_cast<int>(u % sk.num_kb);
-        mbar_wait(&empty_bar[s], ph ^ 1);
+        mbar_wait_mma(&empty_bar[s], ph ^ 1);
         uint8_t* st = smem + s * kStageBytes;
         mbar_arrive_expect_tx(&full_bar[s], kStageBytes);
         tma_load_2d(st, &tmW, &full_bar[s], kb * kBlockK, tile * kBlockN, kEvictFirst);
@@ -124,50 +116,63 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer: one accumulator buffer per segment, alternating =====
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      int seg = 0;
-      long u = u0;
-      while (u < u1) {
-        const int kb_lo = static_cast<int>(u % sk.num_kb);
-        const long rem = u1 - u;
-        const int kb_hi = static_cast<int>((sk.num_kb - kb_lo) < rem ? sk.num_kb : kb_lo + rem);
-        const int buf = seg & 1;
-        mbar_wait(&tmem_empty[buf], ((seg >> 1) & 1) ^ 1);  // the epilogue has drained this buffer (first use passes)
-        tc_fence_after();
-        const uint32_t acc = tmem_base + buf * kBufCols;
-        for (int kb = kb_lo; kb < kb_hi; ++kb) {
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * kStageBytes);
-          const uint32_t b_addr = a_addr + kWTileBytes * kAcc;
-          const uint64_t a_desc = make_kmajor_sw128_desc(a_addr);
-          const uint64_t b_desc = make_kmajor_sw128_desc(b_addr);
-          const uint32_t first = (kb == kb_lo) ? 0u : 1u;
+  } else if (warp < 4) {
+    // ===== MMA warpgroup: one segment at a time, accumulators (both 64-row halves) in registers =====
+    int s = 0;
+    uint32_t ph = 0;
+    int seg = 0;
+    long u = u0;
+    while (u < u1) {
+      const int kb_lo = static_cast<int>(u % sk.num_kb);
+      const long rem = u1 - u;
+      const int kb_hi = static_cast<int>((sk.num_kb - kb_lo) < rem ? sk.num_kb : kb_lo + rem);
+      float acc[2][MPAD / 2], acc2[2][kDual ? MPAD / 2 : 1];
 #pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) umma_f16(acc, a_desc + 2 * k, b_desc + 2 * k, kIdesc, (k > 0) ? 1u : first);
-          if (kDual) {
-            const uint64_t a2_desc = make_kmajor_sw128_desc(a_addr + kWTileBytes);
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k)
-              umma_f16(acc + MPAD, a2_desc + 2 * k, b_desc + 2 * k, kIdesc, (k > 0) ? 1u : first);
-          }
-          umma_commit(&empty_bar[s]);
-          if (++s == stages) {
-            s = 0;
-            ph ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[buf]);
-        u += kb_hi - kb_lo;
-        ++seg;
+        for (int i = 0; i < MPAD / 2; ++i) acc[h][i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < (kDual ? MPAD / 2 : 1); ++i) acc2[h][i] = 0.f;
       }
+      int prev = -1;
+      for (int kb = kb_lo; kb < kb_hi; ++kb) {
+        mbar_wait_mma(&full_bar[s], ph);
+        const uint32_t st = smem_u32(smem + s * kStageBytes);
+        const uint64_t b_desc = make_kmajor_sw128_desc(st + kWTileBytes * kAcc);
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          wgmma_kblock<T, MPAD>(acc[h], make_kmajor_sw128_desc(st + h * (kWTileBytes / 2)), b_desc);
+          if constexpr (kDual) wgmma_kblock<T, MPAD>(acc2[h], make_kmajor_sw128_desc(st + kWTileBytes + h * (kWTileBytes / 2)), b_desc);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its slot can be refilled
+        if (prev >= 0 && threadIdx.x == 0) mbar_arrive(&empty_bar[prev]);
+        prev = s;
+        if (++s == stages) {
+          s = 0;
+          ph ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && threadIdx.x == 0) mbar_arrive(&empty_bar[prev]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        wgmma_fence_acc(acc[h]);
+        wgmma_fence_acc(acc2[h]);
+      }
+      mbar_wait_mma(acc_empty, (seg & 1) ^ 1);  // the epilogue has drained the staging tile (first use passes)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        wgmma_store_acc<MPAD>(acc[h], accbuf, kBlockN, h * 64);
+        if constexpr (kDual) wgmma_store_acc<MPAD>(acc2[h], accbuf + MPAD * kBlockN, kBlockN, h * 64);
+      }
+      mbar_arrive(acc_full);
+      u += kb_hi - kb_lo;
+      ++seg;
     }
   } else {
-    // ===== epilogue warps (TMEM lane quadrant = warp % 4) =====
+    // ===== epilogue warps (thread <-> weight row quad * 32 + lane) =====
     const int quad = warp & 3;
     const int row = quad * 32 + lane;
     pdl_wait();
@@ -180,28 +185,15 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
       const int kb_lo = static_cast<int>(u % sk.num_kb);
       const long rem = u1 - u;
       const int kb_hi = static_cast<int>((sk.num_kb - kb_lo) < rem ? sk.num_kb : kb_lo + rem);
-      const int buf = seg & 1;
       const bool whole = (kb_lo == 0 && kb_hi == sk.num_kb);
-      mbar_wait(&tmem_full[buf], (seg >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + buf * kBufCols + (static_cast<uint32_t>(quad * 32) << 16);
+      mbar_wait_mma(acc_full, seg & 1);
       auto load_chunk = [&](int c, float(&acc)[16], float(&acc2)[16]) {
-        uint32_t r[16];
-        tmem_ld16(taddr + c * 16, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc[j] = __uint_as_float(r[j]);
-        if constexpr (kDual) {
-          tmem_ld16(taddr + MPAD + c * 16, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) acc2[j] = __uint_as_float(r[j]);
-        }
+        acc_ld16(accbuf, kBlockN, row, c * 16, acc);
+        if constexpr (kDual) acc_ld16(accbuf + MPAD * kBlockN, kBlockN, row, c * 16, acc2);
       };
-      auto release_tmem = [&]() {
-        tc_fence_before();
+      auto release_acc = [&]() {
         epi_bar();
-        if (row == 0) mbar_arrive(&tmem_empty[buf]);
+        if (row == 0) mbar_arrive(acc_empty);
       };
       float acc[16], acc2[16];
       if (whole) {
@@ -211,7 +203,7 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
           load_chunk(c, acc, acc2);
           final_chunk<T, EPI>(p, acc, acc2, c * 16, m_valid, row, tile, scratch);
         }
-        release_tmem();
+        release_acc();
       } else {
         // park this segment's fp32 partial in one of the CTA's two workspace slots (a CTA can be contributor of its
         // first tile and finisher of its last one; the two partials must not share storage)
@@ -227,7 +219,7 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
             if constexpr (kDual) __stcg(slot + (MPAD + c * 16 + j) * kBlockN + row, acc2[j]);
           }
         }
-        release_tmem();
+        release_acc();
         if (kb_lo > 0) {
           // contribution: publish and move on (never waits)
           __threadfence();
@@ -240,10 +232,7 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
           if (row == 0) {
             uint32_t spins = 0;
             while (ld_acquire(sk.flags + tile) < expected) {
-              if (++spins > (1u << 26)) {
-                printf("eagle_b200: stream-K finisher timed out (cta %d tile %d)\n", cta, tile);
-                __trap();
-              }
+              if (++spins > (1u << 26)) __trap();  // no printf in a wgmma kernel (see mbar_wait_mma)
             }
             sk.flags[tile] = 0;  // self-reset for the next launch
           }
@@ -273,23 +262,19 @@ skinny_gemm_streamk(const __grid_constant__ CUtensorMap tmW, const __grid_consta
     }
     (void)flag_word;
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<kTmemCols>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------------------
 static int sk_grid_cap() {
-  static int v = 0;
-  if (!v) {
-    const char* e = getenv("EB200_SK_CTAS");  // tuning knob
-    v = e ? atoi(e) : 148;
-    if (v < 1) v = 148;
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("EB200_SK_CTAS");  // tuning knob (default: one CTA per SM)
+    v = e ? atoi(e) : 0;
+    if (v < 1) v = 0;
   }
-  return v;
+  return v ? v : device_sm_count();
 }
 static int sk_smem_kb() {
   static int v = 0;
@@ -302,7 +287,7 @@ static int sk_smem_kb() {
   return v;
 }
 
-size_t streamk_ws_bytes() { return static_cast<size_t>(148) * 2 * 2 * 64 * kBlockN * 4 + 1024; }
+size_t streamk_ws_bytes() { return static_cast<size_t>(device_sm_count()) * 2 * 2 * 64 * kBlockN * 4 + 1024; }
 
 template <typename T, int MPAD, int EPI>
 static int launch_sk_one(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const GemmParams& p,
@@ -317,19 +302,13 @@ static int launch_sk_one(const CUtensorMap* tmW, const CUtensorMap* tmW2, const 
   long g = sk.units / 2;  // at least two k-blocks of work per CTA
   if (g < 1) g = 1;
   if (g > sk_grid_cap()) g = sk_grid_cap();
-  if (g > 148) g = 148;   // workspace slots per CTA; finisher waits need every CTA resident
-  static int n_sm = 0;
-  if (!n_sm) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    if (n_sm < 1) n_sm = 1;
-  }
-  if (g > n_sm) g = n_sm;
-  int stages = (sk_smem_kb() * 1024 - kSkEpiScratch - 512 - 1024) / stage_bytes(MPAD, EPI);
+  if (g > device_sm_count()) g = device_sm_count();  // workspace slots per CTA; finisher waits need every CTA resident
+  constexpr int kFixed = acc_tile_bytes(MPAD, EPI) + kSkEpiScratch + 512 + 1024;
+  int stages = (sk_smem_kb() * 1024 - kFixed) / stage_bytes(MPAD, EPI);
   if (stages > kMaxStages) stages = kMaxStages;
   if (stages < 2) stages = 2;
-  const int smem = stages * stage_bytes(MPAD, EPI) + kSkEpiScratch + 512 + 1024;
+  const int smem = stages * stage_bytes(MPAD, EPI) + kFixed;
+  if (smem > 220 * 1024) return static_cast<int>(cudaErrorInvalidValue);
   static bool configured_dev[64] = {};  // per device (the attribute is per device) and per instantiation
   const int cur_dev = current_device_index();
   if (cur_dev < 0) return static_cast<int>(cudaErrorInvalidDevice);

@@ -88,7 +88,7 @@ struct GemmParams {
 // in a cluster share every X tile, each CTA loads half of it)
 int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX,
                 const GemmParams& p, cudaStream_t s, const CUtensorMap* tmXh = nullptr);
-// bring-up / debugging aid: same epilogues, plain FMA main loop, no TMA/tcgen05.  W/W2/X are raw pointers.
+// bring-up / debugging aid: same epilogues, plain FMA main loop, no TMA/wgmma.  W/W2/X are raw pointers.
 int launch_gemm_simt(int dtype, int mpad, int epi, const void* W, const void* W2, const void* X, long ldx,
                      const GemmParams& p, cudaStream_t s);
 // persistent stream-K variant (gemm_streamk.cu): ws >= streamk_ws_bytes(), flags >= one zeroed int per n-tile
@@ -98,7 +98,7 @@ size_t streamk_ws_bytes();
 // Device table lut[bits(g)] = T(g / (1 + exp(-g))) over all 65536 patterns of the model dtype: the SwiGLU epilogues look the
 // activation up instead of evaluating exp + divide per element (same values by construction).  Built once per device on `s`.
 const void* silu_lut(int dtype, cudaStream_t s);
-// How many bytes of dynamic shared memory / pipeline stages the tcgen05 kernel uses (for reporting)
+// How many bytes of dynamic shared memory / pipeline stages the wgmma kernel uses (for reporting)
 int gemm_stage_count(int mpad, int epi);
 
 // ----------------------------------------------------------------------------------------------
@@ -114,8 +114,8 @@ enum ChainFinish : int {
   FIN_SWIGLU_IL = 1,     // out = T(T(silu(T(gate))) * T(up)) over the interleaved gate/up matrix           (gate_up)
   FIN_QKV_ROPE = 2,      // q -> q_out (rope), k -> K cache (rope), v -> V cache                           (qkv)
   FIN_STORE = 3,         // out = T(acc [+ bias])
-  FIN_ARGMAX = 4,        // whole tiles per CTA, per-tile (max, first index) straight from TMEM, merged per row (verify lm_head)
-  FIN_STORE_DIRECT = 5,  // whole tiles per CTA, out = T(acc [+ bias]) straight from TMEM                  (lm_head, sampling path)
+  FIN_ARGMAX = 4,        // whole tiles per CTA, per-tile (max, first index) from the staged tile, merged per row (verify lm_head)
+  FIN_STORE_DIRECT = 5,  // whole tiles per CTA, out = T(acc [+ bias]) from the staged tile                (lm_head, sampling path)
 };
 constexpr int kChainMaxPhases = 4;
 struct ChainPhase {

@@ -1,29 +1,30 @@
-// Persistent GEMM chain for sm_100a: up to four dependent skinny-M weight-streaming GEMMs in one launch.
+// Persistent GEMM chain for sm_90a: up to four dependent skinny-M weight-streaming GEMMs in one launch.
 //
 // Why: at batch 1 every projection of the verify pass is HBM-bound on its weights, but a chain of ~10 dependent kernels
-// per layer pays a launch/drain/fill bubble of ~10 us around 5-40 us of streaming (DESIGN.md 6: 326 launches per
-// cycle, the small projections at 0.28-0.59 of the HBM roofline).  Here one CTA per SM stays resident for a whole
+// per layer pays a launch/drain/fill bubble around each projection's weight stream (DESIGN.md 10: ~316 launches per
+// cycle).  Here one CTA per SM stays resident for a whole
 // layer segment
 //     o_proj(+residual) -> RMSNorm -> gate/up(SwiGLU) -> down_proj(+residual) -> RMSNorm -> next layer's qkv(+RoPE,+KV append)
 // (or ... -> final norm -> lm_head(arg-max) for the last layer) and
 //   * the WEIGHT producer (one lane) walks the whole task list without ever waiting for a phase boundary: the next
 //     projection's tiles fill the shared-memory ring while the current one is reduced, so HBM never idles;
 //   * every phase is split stream-K style: CTA c owns units [c*U/G, (c+1)*U/G) of the (n-tile, k-block) grid, so all
-//     148 SMs stream the same number of bytes whatever the tile count (32 / 48 / 224 tiles);
-//   * tcgen05.mma accumulates each (tile, k-range) segment in one of two TMEM buffers; the epilogue warps drain it as
-//     an fp32 partial tile into an L2-resident workspace while the next segment's MMAs run;
+//     SMs stream the same number of bytes whatever the tile count (32 / 48 / 224 tiles);
+//   * an MMA warpgroup accumulates each (tile, k-range) segment with wgmma in registers and hands it to the epilogue warps
+//     through a shared-memory staging tile; they drain it as an fp32 partial tile into an L2-resident workspace while the
+//     next segment's MMAs run;
 //   * a global arrival counter per phase replaces the kernel boundary (release/acquire at gpu scope);
 //   * the FINISH step runs row-wise on the first rows*chunks CTAs: fixed-order split-K reduction (deterministic) + the
 //     reference's epilogue arithmetic with its rounding points + the RMSNorm feeding the next phase (the row is complete
 //     inside one CTA, so the norm costs no extra pass, launch or barrier);
 //   * the ACTIVATION producer (another lane) waits for the finish counter of the previous phase and then TMA-loads the
 //     X tiles of its k-blocks behind the already-resident W tiles.
-// The lm_head (1002 tiles) runs in "direct" mode: whole tiles per CTA, per-row (max, first index) straight from TMEM,
+// The lm_head (1002 tiles) runs in "direct" mode: whole tiles per CTA, per-row (max, first index) straight from the staged tile,
 // merged per row in the finish step: the 15.4 MB logits round trip and the arg-max launch disappear.
 //
-// Status (round 2, measured on B200 - DESIGN.md 6, profiles/r02_chain_*): the single-phase lm_head(+arg-max) form is the
-// default; the multi-phase layer chain is parity-green but slower than the per-projection kernels (141 vs ~115 us per
-// 8B layer: the row-wise finish reads its partials through one SM's LSU path), so it stays opt-in (EB200_CHAIN=1).
+// Status (DESIGN.md 6): the single-phase lm_head(+arg-max) form is the default; the multi-phase layer chain is parity-green
+// but its row-wise finish reads the split-K partials through one SM's load/store path, where the per-projection kernels
+// reduce through distributed shared memory, so it stays opt-in (EB200_CHAIN=1).
 //
 // Replaces (per layer) modeling_llama_kv.py:801-863 (decoder layer), :118-132 (RMSNorm), :501-535 (MLP) op sites.
 #include <stdio.h>
@@ -34,7 +35,7 @@
 
 namespace eb {
 
-constexpr int kChainThreads = 256;   // warp0 W producer, warp1 MMA + TMEM, warp2 X producer, warp3 idle, warps 4-7 epilogue/finish
+constexpr int kChainThreads = 320;   // warps 0-3 MMA, warps 4-7 epilogue/finish, warp 8 W producer, warp 9 X producer
 constexpr int kChainMaxSlots = 4;    // partial tiles one CTA may produce per phase
 constexpr int kChainMaxStages = 12;
 constexpr int kChainCtrlBytes = 8192;
@@ -55,15 +56,13 @@ __device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
   asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-// Bounded spin: a mis-programmed chain traps (CUDA error on the host) instead of hanging the box.
-__device__ __forceinline__ void spin_until_ge(const int* p, int target, int what) {
+// Bounded spin: a mis-programmed chain traps (CUDA error on the host) instead of hanging the GPU.  No printf in this kernel:
+// ptxas serialises every wgmma of a kernel in which a call may run while MMAs are in flight (see mbar_wait_mma).
+__device__ __forceinline__ void spin_until_ge(const int* p, int target) {
   uint32_t n = 0;
   while (ld_acquire_gpu(p) < target) {
     __nanosleep(32);
-    if (++n > (1u << 23)) {
-      printf("eagle_b200: chain kernel wait timed out (cta %d, counter %d, have %d, want %d)\n", blockIdx.x, what, ld_acquire_gpu(p), target);
-      __trap();
-    }
+    if (++n > (1u << 23)) __trap();
   }
 }
 __device__ __forceinline__ void chain_epi_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
@@ -85,7 +84,7 @@ __device__ __forceinline__ unsigned long long chain_gtimer() {
 
 // wait for a peer GPU: the peers run the same launch sequence but are not lock-stepped (host launch skew in eager mode), so the
 // bound is wall-clock (20 s), not an iteration count
-__device__ __forceinline__ void spin_until_ge_sys(const int* p, int target, int what) {
+__device__ __forceinline__ void spin_until_ge_sys(const int* p, int target) {
   unsigned long long t0 = 0;
   uint32_t n = 0;
   while (ld_acquire_sys(p) - target < 0) {
@@ -93,11 +92,7 @@ __device__ __forceinline__ void spin_until_ge_sys(const int* p, int target, int 
     if ((++n & 4095u) == 0) {
       const unsigned long long now = chain_gtimer();
       if (!t0) t0 = now;
-      if (now - t0 > 20000000000ull) {
-        printf("eagle_b200: chain kernel timed out waiting for a tensor-parallel peer (cta %d, flag %d, have %d, want %d)\n", blockIdx.x, what,
-               ld_acquire_sys(p), target);
-        __trap();
-      }
+      if (now - t0 > 20000000000ull) __trap();
     }
   }
 }
@@ -211,7 +206,7 @@ __device__ __forceinline__ void build_tile_table(TileSrc* tab, const Geo& g, int
 }
 // sum over all contributors (ascending CTA == ascending k: deterministic) of rows [r, r+4) of tile t, activation row m.
 // The loads of one call are independent and issued back to back (up to 8 in flight): the finish is an L2-latency problem, a
-// load -> add -> load chain costs a full L2 round trip per contributor (measured: 100 us of finish per layer before this).
+// load -> add -> load chain would cost a full L2 round trip per contributor.
 template <int MPAD>
 __device__ __forceinline__ float4 reduce4(const float* ws, const TileSrc* tab, const Geo& g, int G, int t, int m, int r) {
   const TileSrc s = tab[t];
@@ -250,13 +245,11 @@ __device__ __forceinline__ float4 reduce4(const float* ws, const TileSrc* tab, c
   return acc;
 }
 
-// Measured (profiles/r02_chain_phase_trace*.txt): one batch of 24-30 independent 16-byte loads per thread takes ~3 us whatever
-// the load flavour (ld.cg or weak), the run-ahead of the weight ring or L2 prefetching: the LSU path of one SM sustains only
-// ~16 GB/s of L2 reads at this latency (in-flight sectors are bounded), so the row-wise pull-reduce costs 5-15 us per phase.
+// The row-wise pull-reduce is bound by the L2 latency seen by one SM's load/store path (its in-flight sectors are bounded),
+// not by the load flavour (ld.cg or weak): the loads of a batch are therefore all issued before the first add.
 __device__ __forceinline__ float4 ld_partial(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
 // Branch-free batch: NB (tile, row-offset) requests x up to MAXC contributors each, ALL loads issued before the first add.
-// An L2 round trip between SMs costs ~1.3 us under load (phase trace, profiles/r02_chain_phase_trace.txt); the finish must pay
-// it once or twice per item, not once per pass.  Callers check chain_fast_path(g, G, MAXC) (phase-uniform) first.
+// An L2 round trip between SMs is expensive under load; the finish must pay it once or twice per item, not once per pass.  Callers check chain_fast_path(g, G, MAXC) (phase-uniform) first.
 __device__ __forceinline__ bool chain_fast_path(const Geo& g, int G, int maxc) {
   if (g.U < static_cast<uint32_t>(G)) return false;
   const int per = static_cast<int>(g.U / static_cast<uint32_t>(G));
@@ -639,7 +632,7 @@ __device__ __forceinline__ void finish_resid_norm_tp(const ChainPhase& ph, const
   if (etid == 0) st_release_sys(reinterpret_cast<int*>(tp.win[owner] + tp.flag_off) + tp.rank * 64 + m, epoch);
   if (owner != tp.rank) return;  // uniform over the CTA
   // ---- owner: wait for every rank's row, then the single-GPU arithmetic on the fp32 total ----
-  if (etid < tp.size) spin_until_ge_sys(reinterpret_cast<const int*>(tp.win[tp.rank] + tp.flag_off) + etid * 64 + m, epoch, 100 + etid);
+  if (etid < tp.size) spin_until_ge_sys(reinterpret_cast<const int*>(tp.win[tp.rank] + tp.flag_off) + etid * 64 + m, epoch);
   chain_epi_bar();
   __threadfence_system();
   const float* inbox = reinterpret_cast<const float*>(tp.win[tp.rank] + tp.inbox_off) + static_cast<long>(m) * tp.ld_inbox;
@@ -745,7 +738,7 @@ __device__ __forceinline__ void finish_argmax(const ChainPhase& ph, const ChainT
       bv = -INFINITY;
       bi = 0x7fffffff;
       for (int src = 0; src < tp.size; ++src) {
-        spin_until_ge_sys(flags + src * 64 + m, epoch, 200 + src);
+        spin_until_ge_sys(flags + src * 64 + m, epoch);
         const float v = __ldcg(mine + (static_cast<long>(src) * 64 + m) * 2);
         const int i = __ldcg(reinterpret_cast<const int*>(mine + (static_cast<long>(src) * 64 + m) * 2) + 1);
         if (better(v, i, bv, bi)) {
@@ -767,8 +760,6 @@ __global__ void __launch_bounds__(kChainThreads, 1)
 gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ ChainArgs args, const int stages) {
   constexpr int kXBytes = x_tile_bytes(MPAD);
   constexpr int kStageBytes = kWTileBytes + kXBytes;
-  constexpr int kTmemCols = (2 * MPAD < 32) ? 32 : 2 * MPAD;
-  constexpr uint32_t kIdesc = make_idesc_f16<T>(kBlockN, MPAD);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -776,9 +767,9 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
   uint64_t* fullW = reinterpret_cast<uint64_t*>(ctrl);
   uint64_t* fullX = fullW + kChainMaxStages;
   uint64_t* empty = fullX + kChainMaxStages;
-  uint64_t* tmem_full = empty + kChainMaxStages;  // [2]
-  uint64_t* tmem_empty = tmem_full + 2;           // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* acc_full = empty + kChainMaxStages;   // the staging tile holds a segment's accumulators (128 arrivals)
+  uint64_t* acc_empty = acc_full + 1;             // the epilogue has drained it
+  float* accbuf = reinterpret_cast<float*>(ctrl + kChainCtrlBytes);  // [MPAD][128] staged fp32 accumulators
   float* red = reinterpret_cast<float*>(ctrl + 512);                // [4] block-sum scratch, then [4][64] arg-max pairs
   float* sval = reinterpret_cast<float*>(ctrl + 1024);              // [4][64]
   int* sidx = reinterpret_cast<int*>(ctrl + 1024 + 4 * 64 * 4);     // [4][64]
@@ -799,20 +790,13 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
       mbar_init(&fullX[i], 1);
       mbar_init(&empty[i], 1);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 1);
-    }
+    mbar_init(acc_full, 128);
+    mbar_init(acc_empty, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<kTmemCols>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(smem_u32(tmem_ptr)));
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===== weight producer: the whole task list, never blocked by a phase boundary (weights depend on nothing).  While the
     // ring is full (the MMA side waits for a finish step) a second cursor keeps HBM busy: it prefetches the next l2_window weight
     // tiles into L2, from where the ring refills faster than from HBM once the MMAs resume. =====
@@ -826,9 +810,9 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
       pf = ld;
       int ahead = 0;  // units the prefetch cursor is ahead of the load cursor
       const int window = args.l2_window;
-      // Run-ahead throttle: the finish of phase p reads ~5 MB of partials through the same L2 / die-to-die fabric the weight
-      // stream saturates; letting the ring refill at full speed during the finish stretches the (critical-path) finish from
-      // ~3 to ~13 us (phase trace).  So only w_ahead tiles of phase p+1 are fetched before ready[p] is observed.
+      // Run-ahead throttle: the finish of phase p reads ~5 MB of partials through the same L2 the weight stream saturates;
+      // letting the ring refill at full speed during the finish can stretch the (critical-path) finish.  So only w_ahead tiles
+      // of phase p+1 are fetched before ready[p] is observed (EB200_CHAIN_W_AHEAD; default -1 = no throttle).
       int cur_phase = ld.done ? 0 : ld.p, into_phase = 0;
       bool prev_ready = true;
       int m_valid_w = -1;
@@ -850,9 +834,9 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
           if (args.tp.size > 1 && prev.fin == FIN_RESID_NORM) {
             int seen = 0;
             for (int q = 0; q < cur_phase; ++q) seen += args.ph[q].fin == FIN_RESID_NORM ? 1 : 0;
-            spin_until_ge_sys(reinterpret_cast<const int*>(args.tp.win[args.tp.rank] + args.tp.ready_off), tp_ready0_w + seen * m_valid_w, 400 + cur_phase);
+            spin_until_ge_sys(reinterpret_cast<const int*>(args.tp.win[args.tp.rank] + args.tp.ready_off), tp_ready0_w + seen * m_valid_w);
           } else {
-            spin_until_ge(args.sync + kSyncReady + (cur_phase - 1), m_valid_w * prev.chunks, 20 + cur_phase);
+            spin_until_ge(args.sync + kSyncReady + (cur_phase - 1), m_valid_w * prev.chunks);
           }
           prev_ready = true;
         }
@@ -864,7 +848,6 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
             cursor_advance(pf, args, cta, G);
             ++ahead;
           } else if (++spins > (1u << 26)) {
-            printf("eagle_b200: chain weight producer timed out (block %d)\n", blockIdx.x);
             __trap();
           }
         }
@@ -879,7 +862,7 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
         }
       }
     }
-  } else if (warp == 2) {
+  } else if (warp == 9) {
     // ===== activation producer: X tiles of phase p exist once finish(p-1) has completed (phase 0: the previous kernel) =====
     if (lane == 0) {
       pdl_wait();
@@ -894,16 +877,16 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
           if (args.tp.size > 1 && prev.fin == FIN_RESID_NORM) {
             // rows of this phase's X operand are pushed by their owners on all ranks (finish_resid_norm_tp)
             tp_resid_seen += 1;
-            spin_until_ge_sys(reinterpret_cast<const int*>(args.tp.win[args.tp.rank] + args.tp.ready_off), tp_ready0 + tp_resid_seen * m_valid, 300 + p);
+            spin_until_ge_sys(reinterpret_cast<const int*>(args.tp.win[args.tp.rank] + args.tp.ready_off), tp_ready0 + tp_resid_seen * m_valid);
           } else {
-            spin_until_ge(args.sync + kSyncReady + (p - 1), m_valid * prev.chunks, kSyncReady + p - 1);
+            spin_until_ge(args.sync + kSyncReady + (p - 1), m_valid * prev.chunks);
           }
           fence_proxy_async_all();  // generic-proxy writes of other SMs (acquired above) -> this thread's async-proxy (TMA) reads
         }
         const Geo g = geo_of(args.ph[p]);
         for_each_segment(g, cta, G, [&](int, int a, int b, int) {
           for (int kb = a; kb < b; ++kb) {
-            mbar_wait(&empty[s], par ^ 1);
+            mbar_wait_mma(&empty[s], par ^ 1);
             mbar_arrive_expect_tx(&fullX[s], kXBytes);
             tma_load_2d(smem + s * kStageBytes + kWTileBytes, &maps.x[p], &fullX[s], kb * kBlockK, 0, kEvictLast);
             if (++s == stages) {
@@ -914,50 +897,60 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
         });
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      int s = 0;
-      uint32_t par = 0, seg = 0;
-      unsigned long long* trc = args.trace ? args.trace + 32ull * cta : nullptr;
-      for (int p = 0; p < args.n_phases; ++p) {
-        const Geo g = geo_of(args.ph[p]);
-        bool first = true;
-        for_each_segment(g, cta, G, [&](int, int a, int b, int) {
-          const uint32_t buf = seg & 1, use = seg >> 1;
-          mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);  // the epilogue has drained this accumulator
-          tc_fence_after();
-          const uint32_t d_addr = tmem_base + buf * MPAD;
-          for (int kb = a; kb < b; ++kb) {
-            mbar_wait(&fullW[s], par);
-            mbar_wait(&fullX[s], par);
-            if (trc && first) {
-              trc[1 + 6 * p + 4] = chain_gtimer();  // first X tile of the phase has landed
-              first = false;
-            }
-            tc_fence_after();
-            const uint32_t a_addr = smem_u32(smem + s * kStageBytes);
-            const uint64_t a_desc = make_kmajor_sw128_desc(a_addr);
-            const uint64_t b_desc = make_kmajor_sw128_desc(a_addr + kWTileBytes);
+  } else if (warp < 4) {
+    // ===== MMA warpgroup: both 64-row halves of each tile, fp32 accumulators in registers =====
+    const bool lead = threadIdx.x == 0;
+    int s = 0;
+    uint32_t par = 0, seg = 0;
+    unsigned long long* trc = (args.trace && lead) ? args.trace + 32ull * cta : nullptr;
+    for (int p = 0; p < args.n_phases; ++p) {
+      const Geo g = geo_of(args.ph[p]);
+      bool first = true;
+      for_each_segment(g, cta, G, [&](int, int a, int b, int) {
+        float acc[2][MPAD / 2];
 #pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k) umma_f16(d_addr, a_desc + 2 * k, b_desc + 2 * k, kIdesc, (k > 0 || kb > a) ? 1u : 0u);
-            umma_commit(&empty[s]);
-            if (++s == stages) {
-              s = 0;
-              par ^= 1;
-            }
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < MPAD / 2; ++i) acc[h][i] = 0.f;
+        int prev = -1;
+        for (int kb = a; kb < b; ++kb) {
+          mbar_wait_mma(&fullW[s], par);
+          mbar_wait_mma(&fullX[s], par);
+          if (trc && first) {
+            trc[1 + 6 * p + 4] = chain_gtimer();  // first X tile of the phase has landed
+            first = false;
           }
-          umma_commit(&tmem_full[buf]);
-          ++seg;
-        });
-        if (trc) trc[1 + 6 * p + 5] = chain_gtimer();  // last MMA of the phase issued
-      }
+          const uint32_t st = smem_u32(smem + s * kStageBytes);
+          const uint64_t b_desc = make_kmajor_sw128_desc(st + kWTileBytes);
+          wgmma_fence();
+#pragma unroll
+          for (int h = 0; h < 2; ++h) wgmma_kblock<T, MPAD>(acc[h], make_kmajor_sw128_desc(st + h * (kWTileBytes / 2)), b_desc);
+          wgmma_commit();
+          wgmma_wait<1>();  // the previous k-block's MMAs have retired: its slot can be refilled
+          if (prev >= 0 && lead) mbar_arrive(&empty[prev]);
+          prev = s;
+          if (++s == stages) {
+            s = 0;
+            par ^= 1;
+          }
+        }
+        wgmma_wait<0>();
+        if (prev >= 0 && lead) mbar_arrive(&empty[prev]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) wgmma_fence_acc(acc[h]);
+        mbar_wait_mma(acc_empty, (seg & 1) ^ 1);  // the epilogue has drained the staging tile (first use passes)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) wgmma_store_acc<MPAD>(acc[h], accbuf, kBlockN, h * 64);
+        mbar_arrive(acc_full);
+        ++seg;
+      });
+      if (trc) trc[1 + 6 * p + 5] = chain_gtimer();  // last MMA of the phase issued
     }
   } else if (warp >= 4) {
-    // ===== epilogue + finish warps (TMEM lane quadrant = warp % 4) =====
+    // ===== epilogue + finish warps (thread <-> weight row quad * 32 + lane) =====
     const int quad = warp & 3;
     const int etid = threadIdx.x - 128;
-    const int row = quad * 32 + lane;  // weight row inside the tile == TMEM lane
+    const int row = quad * 32 + lane;  // weight row inside the tile
     pdl_wait();
     const int m_valid = args.m_idx >= 0 ? min(args.m_rows, ld_dep(args.st + args.m_idx)) : args.m_rows;
     if (args.timing && cta == 0 && etid == 0) *reinterpret_cast<volatile unsigned long long*>(args.timing + 2) = chain_gtimer();
@@ -971,25 +964,21 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
       const Geo g = geo_of(ph);
       bool first_seg = true;
       for_each_segment(g, cta, G, [&](int t, int, int, int slot) {
-        const uint32_t buf = seg & 1, use = seg >> 1;
-        mbar_wait(&tmem_full[buf], use & 1);
+        mbar_wait_mma(acc_full, seg & 1);
         if (tre && first_seg) {
           tre[1 + 6 * p + 0] = chain_gtimer();  // first accumulator of the phase complete
           first_seg = false;
         }
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + buf * MPAD;
         if (!g.direct) {
           float* part = my_ws + static_cast<long>(slot) * MPAD * kBlockN + row;
 #pragma unroll 1
           for (int c = 0; c < MPAD / 16; ++c) {
             if (c * 16 >= m_valid) break;
-            uint32_t r[16];
-            tmem_ld16(taddr + c * 16, r);
-            tmem_ld_wait();
+            float r[16];
+            acc_ld16(accbuf, kBlockN, row, c * 16, r);
 #pragma unroll
             for (int j = 0; j < 16; ++j)
-              if (c * 16 + j < m_valid) __stcg(part + (c * 16 + j) * kBlockN, __uint_as_float(r[j]));
+              if (c * 16 + j < m_valid) __stcg(part + (c * 16 + j) * kBlockN, r[j]);
           }
         } else if (ph.fin == FIN_STORE_DIRECT) {
           GemmParams gp;
@@ -1001,11 +990,10 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
 #pragma unroll 1
           for (int c = 0; c < MPAD / 16; ++c) {
             if (c * 16 >= m_valid) break;
-            uint32_t r[16];
-            tmem_ld16(taddr + c * 16, r);
-            tmem_ld_wait();
+            float r[16];
+            acc_ld16(accbuf, kBlockN, row, c * 16, r);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) acc[j] = acc2[j] = __uint_as_float(r[j]);
+            for (int j = 0; j < 16; ++j) acc[j] = acc2[j] = r[j];
             final_chunk<T, EPI_STORE>(gp, acc, acc2, c * 16, m_valid, row, t, nullptr);
           }
         } else {  // FIN_ARGMAX: per-row (max, first index) of this tile's 128 vocabulary rows
@@ -1013,12 +1001,11 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
 #pragma unroll 1
           for (int c = 0; c < MPAD / 16; ++c) {
             if (c * 16 >= m_valid) break;
-            uint32_t r[16];
-            tmem_ld16(taddr + c * 16, r);
-            tmem_ld_wait();
+            float r[16];
+            acc_ld16(accbuf, kBlockN, row, c * 16, r);
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
-              float v = (n < ph.N) ? rnd<T>(__uint_as_float(r[j])) : -INFINITY;  // the logits tensor is model dtype (ea_model.py:190)
+              float v = (n < ph.N) ? rnd<T>(r[j]) : -INFINITY;  // the logits tensor is model dtype (ea_model.py:190)
               int idx = n;
 #pragma unroll
               for (int o = 16; o > 0; o >>= 1) {
@@ -1049,9 +1036,8 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
             __stcg(ph.tile_idx + static_cast<long>(t) * 64 + etid, bi);
           }
         }
-        tc_fence_before();
-        chain_epi_bar();  // every epilogue thread is done with this TMEM buffer (and with sval/sidx)
-        if (etid == 0) mbar_arrive(&tmem_empty[buf]);
+        chain_epi_bar();  // every epilogue thread is done with the staging tile (and with sval/sidx)
+        if (etid == 0) mbar_arrive(acc_empty);
         ++seg;
       });
       // ---- all partials / tile results of this CTA for phase p are written ----
@@ -1063,7 +1049,7 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
         if (etid == 0 && cta < m_valid * ph.chunks) {
           int mine = 0;
           for (int it = cta; it < m_valid * ph.chunks; it += G) ++mine;
-          spin_until_ge(args.sync + kSyncPartials + p, G, kSyncPartials + p);
+          spin_until_ge(args.sync + kSyncPartials + p, G);
           red_release_gpu_add(args.sync + kSyncReady + p, mine);
         }
         continue;
@@ -1072,7 +1058,7 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
       const int n_items = m_valid * ph.chunks;
       if (cta < n_items) {
         if (!g.direct) build_tile_table(tab, g, G, etid);
-        if (etid == 0) spin_until_ge(args.sync + kSyncPartials + p, G, kSyncPartials + p);
+        if (etid == 0) spin_until_ge(args.sync + kSyncPartials + p, G);
         chain_epi_bar();
         __threadfence();
         if (tre) tre[1 + 6 * p + 2] = chain_gtimer();  // every CTA's partials have arrived: finish starts
@@ -1103,9 +1089,7 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant_
     if (tre) tre[31] = chain_gtimer();
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc<kTmemCols>(tmem_base);
   if (threadIdx.x == 0) {
     pdl_wait();  // (returns at once: the epilogue warps already waited) keeps every global access of this thread behind the wait
     // the last CTA to leave resets the counters for the next launch on this stream (nobody polls after its own exit ticket)
@@ -1183,14 +1167,15 @@ template <typename T, int MPAD> static int launch_chain_t(const ChainMaps& maps,
   const int G = chain_grid_for(dev);
   if (G <= 0) return static_cast<int>(cudaErrorInvalidDevice);
   constexpr int kStageBytes = kWTileBytes + x_tile_bytes(MPAD);
+  constexpr int kAccBytes = MPAD * kBlockN * 4;
   const int max_smem = 227 * 1024;
-  int stages = (max_smem - 1024 - kChainCtrlBytes) / kStageBytes;
+  int stages = (max_smem - 1024 - kChainCtrlBytes - kAccBytes) / kStageBytes;
   if (stages > kChainMaxStages) stages = kChainMaxStages;
   {
     const char* e = getenv("EB200_CHAIN_STAGES");
     if (e && atoi(e) >= 2 && atoi(e) < stages) stages = atoi(e);
   }
-  const size_t smem = static_cast<size_t>(stages) * kStageBytes + kChainCtrlBytes + 1024;
+  const size_t smem = static_cast<size_t>(stages) * kStageBytes + kChainCtrlBytes + kAccBytes + 1024;
   static bool configured[64] = {};  // per device (and per instantiation: this is a template)
   if (!configured[dev]) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
@@ -1206,7 +1191,7 @@ int launch_gemm_chain(int dtype, int mpad, const ChainMaps& maps, const ChainArg
     static int window = -1;
     if (window < 0) {
       const char* e = getenv("EB200_CHAIN_L2_WINDOW");
-      window = e ? atoi(e) : 0;  // measured (profiles/r02_chain_prefetch_ab.txt): prefetch traffic slows the finish reads more than it saves
+      window = e ? atoi(e) : 0;  // off by default: prefetch traffic competes with the finish reads
       if (window < 0) window = 0;
       if (window > 256) window = 256;
     }

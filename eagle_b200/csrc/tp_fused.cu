@@ -1,7 +1,7 @@
 // Tensor-parallel "all-reduce + residual + RMSNorm" in ONE kernel over NVLink peer memory (no NCCL on the decode path).
 //
 // A row-parallel projection (o_proj, down_proj: modeling_llama_kv.py:768, :838-845) leaves an unrounded fp32 partial
-// [rows][H] on every rank (gemm.cu EPI_PARTIAL_F32).  Round 1 then ran ncclAllReduce (983 KB, latency-bound, ~15-20 us) ->
+// [rows][H] on every rank (gemm.cu EPI_PARTIAL_F32).  The NCCL path runs ncclAllReduce (983 KB, latency-bound) ->
 // residual_add_f32 -> rmsnorm: three launches per projection, 64 projections per verify pass.  Here one CTA per row does a
 // ONE-SHOT exchange (one NVLink hop, no reduce-scatter/all-gather round trip):
 //   A. pushes its rank's fp32 row into inbox[epoch parity][rank][row] of EVERY rank's peer window (plain 16-byte stores over
@@ -174,7 +174,7 @@ __global__ void __launch_bounds__(kTpThreads) tp_resid_norm_kernel(const TpResid
 }
 
 // Two-shot variant for large tp (reduce-scatter + all-gather by rows): the one-shot kernel pushes (tp-1) x 16 KB per row and
-// rank -- 6.9 MB per projection at tp = 8, ~8 us of NVLink time, and every CTA waits for 8 flags.  Here row m is reduced only on
+// rank -- 6.9 MB per projection at tp = 8, and every CTA waits for 8 flags.  Here row m is reduced only on
 // its owner (m % tp): every rank pushes the row to the owner (1.7 MB per projection at tp = 8), the owner finishes it and pushes
 // the bf16 x / xn (/ tap) rows to every rank, then raises a per-row flag there; a CTA leaves when its row has arrived locally.
 template <typename T>
@@ -305,7 +305,7 @@ int launch_tp_resid_norm(int dtype, const TpResidParams& p, int rows, cudaStream
   static int two_shot_min = -1;  // smallest tp that uses the two-shot exchange (EB200_TP_TWO_SHOT_MIN)
   if (two_shot_min < 0) {
     const char* e = getenv("EB200_TP_TWO_SHOT_MIN");
-    two_shot_min = e ? atoi(e) : 8;  // measured at tp = 8: 185.6 vs 176.0 tok/s (profiles/r02_bench_tp8_two_shot.json); one-shot verified at tp = 2 and 8
+    two_shot_min = e ? atoi(e) : 8;  // from 8 ranks the one-shot volume ((tp-1) x 16 KB per row and rank) dominates
     if (two_shot_min < 2) two_shot_min = 2;
   }
   if (p.tp.size >= two_shot_min) {

@@ -1,10 +1,10 @@
-"""`EaModel`: the reference's public API (eagle/model/ea_model.py:25-558) over the B200 engine.
+"""`EaModel`: the reference's public API (eagle/model/ea_model.py:25-558) over the H100 engine.
 
 Same constructor arguments, method names, argument meanings, return conventions and
 checkpoint format as the reference, so callers (`gen_ea_answer_*.py`, `webui.py`) switch by
 changing one import.  Everything between the arguments and the returned ids -- prefill, draft
 tree growth, tree-masked verification, posterior acceptance, KV compaction -- runs inside
-libeagle_b200.so (hand-written sm_100a CUDA); torch is used here only to hold the caller's
+libeagle_b200.so (hand-written sm_90a CUDA); torch is used here only to hold the caller's
 tensors and to read checkpoints.  There is no PyTorch / CPU fallback path.
 """
 from __future__ import annotations
@@ -283,7 +283,7 @@ class EaModel(torch.nn.Module):
         if any(kwargs.get(k) for k in ("load_in_8bit", "load_in_4bit")):
             raise ValueError("eagle_b200 runs bf16 / fp16 weights; quantised loading is not supported")
         if ignored:
-            warnings.warn(f"eagle_b200 places the whole model on one B200 (`device`); ignoring {ignored}", stacklevel=2)
+            warnings.warn(f"eagle_b200 places the whole model on one GPU (`device`); ignoring {ignored}", stacklevel=2)
         tc = read_json(os.path.join(base_model_path, "config.json"))
         if tc.get("architectures", ["LlamaForCausalLM"])[0] != "LlamaForCausalLM":
             raise ValueError("eagle_b200 supports Llama-family targets (the configs named in BASELINE.json)")

@@ -1,5 +1,5 @@
 """Tensor-parallel plumbing: one process per GPU (torchrun), torch.distributed only carries the 128-byte NCCL unique id;
-the collectives themselves are issued by libeagle_b200.so on its own stream (NCCL over NVLink 5 / NVSwitch).
+the collectives themselves are issued by libeagle_b200.so on its own stream (NCCL over NVLink / NVSwitch).
 
 The reference has no tensor parallelism (its multi-GPU mode is accelerate layer placement, ea_model.py:104-118);
 sharding follows the usual column/row-parallel split of a Llama block (SURVEY.md 8e): q/k/v by heads and gate/up by rows,

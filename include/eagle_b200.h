@@ -1,4 +1,4 @@
-/* eagle_b200 -- C ABI of the B200-native EAGLE speculative-decoding engine.
+/* eagle_b200 -- C ABI of the H100-native EAGLE speculative-decoding engine.
  *
  * The reference (SafeAILab/EAGLE) has no FFI layer: its drop-in boundary is the Python surface of
  * `EaModel` (eagle/model/ea_model.py:25-558).  This library is what a thin `EaModel`-compatible class binds

@@ -1,7 +1,7 @@
 """Torch-CPU restatement of the reference's draft -> verify -> accept hot path.
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  Every function cites the reference
-file:line (under /root/reference/eagle/model/) whose arithmetic it restates.  The
+file:line (under eagle/model/ of the reference) whose arithmetic it restates.  The
 restatement keeps the reference's *rounding points* (which intermediate is rounded to
 the model dtype, which is kept in fp32) because those decide the bf16/fp16 results:
 

@@ -1,6 +1,6 @@
 """Generate tests/golden/*.pt by running the UNMODIFIED reference on CPU.
 
-Runs only in the build container (needs /root/reference; the GPU box has no reference).
+Needs a checkout of the reference, its root in the EAGLE_REFERENCE environment variable; no test runs it.
 The reference is imported with three environment shims that live here, not in the
 reference (SURVEY.md 8c): (1) stub eagle.model.modeling_qwen3_kv (does not import on
 transformers 5.x), (2) reset rope_scaling=None + rope_theta on configs, (3) bypass hub /
@@ -22,13 +22,15 @@ import types
 import torch
 import torch.nn as nn
 
-REF = "/root/reference"
+REF = os.environ.get("EAGLE_REFERENCE", "")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 GOLD = os.path.join(ROOT, "tests", "golden")
 
 
 def import_reference():
+    if not REF or not os.path.isdir(os.path.join(REF, "eagle")):
+        raise SystemExit("set EAGLE_REFERENCE to the root of a SafeAILab/EAGLE checkout")
     sys.dont_write_bytecode = True
     sys.path.insert(0, REF)
     stub = types.ModuleType("eagle.model.modeling_qwen3_kv")
@@ -278,6 +280,11 @@ def make_static_goldens():
     print("wrote", out, os.path.getsize(out), "bytes")
 
 
+# Fixtures whose float hidden-state captures (trees[*].in_hidden, cycles[*].hidden_new) no test reads: they are dropped so
+# that the stored file stays small (the tensor-parallel fixture is wide; with them it exceeds 1 MB).
+LEAN_FIXTURES = {"e3_tp8_bf16"}
+
+
 def main():
     os.makedirs(GOLD, exist_ok=True)
     torch.set_num_threads(max(1, os.cpu_count() or 1))
@@ -301,6 +308,11 @@ def main():
         m, em = build_reference_model(tcfg, tW, hcfg, hW, eagle3, dtype, **tree)
         prompt = make_prompt(tcfg["vocab_size"], plen, pseed)
         rec = run_and_capture(m, em, prompt, sampling_seed=sseed, **gen_kw)
+        if fx in LEAN_FIXTURES:
+            for t in rec["trees"]:
+                t.pop("in_hidden")
+            for c in rec["cycles"]:
+                c.pop("hidden_new")
         naive = m.naivegenerate(prompt, temperature=0.0, max_new_tokens=gen_kw["max_new_tokens"],
                                 max_length=gen_kw["max_length"]) if sseed is None else None
         rec["naive_ids"] = naive

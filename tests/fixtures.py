@@ -1,6 +1,7 @@
 """Shared helpers: build the named tiny fixtures for the oracle and for the CUDA engine."""
 import os
 import random
+import tempfile
 
 import torch
 
@@ -8,6 +9,17 @@ from oracle import eagle_oracle as orc
 from oracle.make_golden import FIXTURES, STOP_FIXTURES, base_fixture, fixture_models, make_prompt
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+# informational parity notes of the GPU tests (what agreed with the reference and how closely), outside the source tree
+REPORT = os.path.join(tempfile.gettempdir(), "eagle_b200_parity_report.txt")
+_report_started = False
+
+
+def report(line: str):
+    """Add one line to REPORT; the first call of a test process starts the file afresh."""
+    global _report_started
+    with open(REPORT, "a" if _report_started else "w") as f:
+        f.write(line + "\n")
+    _report_started = True
 
 
 def load_golden(name):

@@ -1,4 +1,4 @@
-"""Parity of the persistent per-layer chain kernel (eagle_b200/csrc/mega.cu) on the B200, through the C ABI.
+"""Parity of the persistent per-layer chain kernel (eagle_b200/csrc/mega.cu) on the H100, through the C ABI.
 
 The kernel replaces, per decoder layer, modeling_llama_kv.py:801-863 (o_proj + residual, post-attention RMSNorm, SwiGLU MLP,
 down_proj + residual, the next block's input RMSNorm and qkv projection with RoPE + KV append) and, after the last layer,

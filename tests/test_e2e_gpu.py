@@ -1,4 +1,4 @@
-"""End-to-end parity on the B200: the CUDA engine behind `EaModel` against the reference-generated
+"""End-to-end parity on the H100: the CUDA engine behind `EaModel` against the reference-generated
 golden vectors (tests/golden, produced by the unmodified reference) and the CPU oracle.
 
 Bar (north star): identical accepted-token sequences under greedy decoding.  Greedy speculative decoding
@@ -7,13 +7,12 @@ tree-attention forward.  On the correlated fixtures (peaked distributions, large
 accept lengths and trees must match the reference exactly; on random-weight fixtures (near-uniform logits,
 bf16 top-2 margins below summation-order noise) we require the first cycles to match and report the rest.
 """
-import os
 
 import pytest
 import torch
 
 from oracle.make_golden import FIXTURES, fixture_models
-from tests.fixtures import build_oracle, load_golden
+from tests.fixtures import build_oracle, load_golden, report
 
 pytestmark = pytest.mark.gpu
 
@@ -53,7 +52,7 @@ def build_engine(fx, flags=0, max_length=512):
     return m, dtype
 
 
-@pytest.mark.parametrize("flags", [1, 0], ids=["simt-gemm", "tcgen05"])
+@pytest.mark.parametrize("flags", [1, 0], ids=["simt-gemm", "wgmma"])
 @pytest.mark.parametrize("fx", ["e3_corr_bf16", "e1_corr_fp16", "e3_gqa_bf16"])
 def test_correlated_fixture_identical_to_reference(fx, flags):
     g = load_golden(fx)
@@ -81,9 +80,7 @@ def test_first_tree_and_stepwise_state(fx):
     assert dt.shape == t0["draft_tokens"].shape and int(dt[0, 0]) == int(t0["draft_tokens"][0, 0])
     assert bool((tm[0, 0].diagonal() == 1).all()) and bool((tm[0, 0, :, 0] == 1).all())
     shared = len(set(ours) & set(ref))
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/parity_report.txt", "a") as f:
-        f.write(f"{fx}: first tree shares {shared}/{len(ref)} root->node paths with the reference tree\n")
+    report(f"{fx}: first tree shares {shared}/{len(ref)} root->node paths with the reference tree")
     if corr:
         gc0 = g["cycles"][0]
         accepted = tuple(gc0["candidates"][gc0["best"], : gc0["accept_length"] + 1].tolist())
@@ -148,10 +145,8 @@ def test_random_weights_lossless_and_reported(fx):
     margin_ulps = (top2[:, 0] - top2[:, 1]) / spacing
     fragile = (margin_ulps < 2.0).nonzero().flatten()
     must_match = int(fragile[0]) if fragile.numel() else k - P
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/parity_report.txt", "a") as f:
-        f.write(f"{fx}: identical generated-token prefix vs reference {agree - P}/{k - P}; first sub-2-ulp decision of the reference at "
-                f"generated token {must_match} (min margin {float(margin_ulps.min()):.2f} ulp)\n")
+    report(f"{fx}: identical generated-token prefix vs reference {agree - P}/{k - P}; first sub-2-ulp decision of the reference at "
+           f"generated token {must_match} (min margin {float(margin_ulps.min()):.2f} ulp)")
     assert agree - P >= must_match, f"diverged at generated token {agree - P}, before the first fragile decision ({must_match})"
 
 
@@ -216,8 +211,7 @@ def test_sampling_posterior_is_lossless_monte_carlo():
         counts[bucket_of[int(ids[0, P + 1])]] += 1
         accepted_second += int(new_token > idx + 1)
     chi2 = float(((counts - expected) ** 2 / expected).sum())
-    with open("gpurun_out/parity_report.txt", "a") as f:
-        f.write(f"sampling losslessness: chi2={chi2:.1f} over {n_buckets} equal-mass buckets, {n_trials} trials\n")
+    report(f"sampling losslessness: chi2={chi2:.1f} over {n_buckets} equal-mass buckets, {n_trials} trials")
     assert chi2 < 45.0, f"second-token histogram deviates from the target distribution: chi2={chi2:.1f} (df=15)"
 
 

@@ -8,13 +8,12 @@ Checked: committed ids, (new_token, idx), per-cycle accept lengths and committed
 that both trees contain, and the DRAFT LOGITS of the last tree level (north star: within 1e-3 at bf16 -- read as 1e-3 absolute
 plus one ulp of the model dtype, the spacing of the tensor the reference itself materialises).
 """
-import os
 
 import pytest
 import torch
 
 from oracle import eagle_oracle as orc
-from tests.fixtures import to_cfg
+from tests.fixtures import report, to_cfg
 from tests.test_e2e_gpu import node_map
 
 pytestmark = pytest.mark.gpu
@@ -106,7 +105,5 @@ def test_draft_logits_within_1e3_of_the_oracle(pair):
         n_bad += int((err > tol).sum())
         n_all += err.numel()
         worst = max(worst, float((err / (1e-3 + ULP_BF16 * want[j].abs())).max()))
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/parity_report.txt", "a") as f:
-        f.write(f"full-shape draft logits ({len(pairs)} comparable frontier rows): {n_bad}/{n_all} elements beyond 1e-3 + 1 ulp; worst error {worst:.2f} x tolerance\n")
+    report(f"full-shape draft logits ({len(pairs)} comparable frontier rows): {n_bad}/{n_all} elements beyond 1e-3 + 1 ulp; worst error {worst:.2f} x tolerance")
     assert n_bad <= n_all * 1e-3 and worst <= 3.0, f"{n_bad}/{n_all} draft logits beyond 1e-3 + 1 bf16 ulp; worst {worst:.2f}x"

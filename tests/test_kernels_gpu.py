@@ -1,4 +1,4 @@
-"""Per-kernel parity on the B200: every CUDA kernel is called in isolation through the C ABI
+"""Per-kernel parity on the H100: every CUDA kernel is called in isolation through the C ABI
 (eb200_k_* entry points) and compared with the CPU oracle's arithmetic on the same seeded inputs.
 
 Tolerances (written here, per the north star): integer/index outputs are bit-exact; floating-point
@@ -58,7 +58,7 @@ def ptr(t):
 
 
 # ----------------------------------------------------------------------------------------------
-# skinny GEMM (tcgen05 + TMA) and its epilogues
+# skinny GEMM (wgmma + TMA) and its epilogues
 # ----------------------------------------------------------------------------------------------
 GEMM_CASES = [
     # M, N, K, splitk

@@ -1,8 +1,7 @@
-"""Static draft tree on the B200 (SURVEY.md 8 row a11): the engine's fixed-tree mode against the CPU oracle
+"""Static draft tree on the H100 (SURVEY.md 8 row a11): the engine's fixed-tree mode against the CPU oracle
 (oracle/static_tree.py, pinned bit-for-bit on the reference's own buffers / generate_candidates / EAGLEModel.topK_genrate
 by tests/test_static_tree_cpu.py) and against reference-generated goldens where the kernel has one."""
 import ctypes as C
-import os
 
 import pytest
 import torch
@@ -10,7 +9,7 @@ import torch
 from oracle import eagle_oracle as orc
 from oracle import static_tree as stt
 from oracle.make_golden import fixture_models, make_prompt
-from tests.fixtures import load_golden, to_cfg
+from tests.fixtures import load_golden, report, to_cfg
 
 pytestmark = pytest.mark.gpu
 
@@ -112,9 +111,7 @@ def test_static_generation_identical_to_oracle(fx, topk):
             oc["best"], : oc["accept_length"] + 1].tolist()
         assert toks == want, f"cycle {c}: committed {toks} != oracle {want}"
         assert acc == oc["accept_length"] and nxt == oc["bonus"]
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/parity_report.txt", "a") as f:
-        f.write(f"static {fx} top_k={topk}: {same}/{total} tree tokens (nodes with identical ancestors) identical to the oracle over {len(o.cycle_log)} cycles\n")
+    report(f"static {fx} top_k={topk}: {same}/{total} tree tokens (nodes with identical ancestors) identical to the oracle over {len(o.cycle_log)} cycles")
     # first-divergence nodes are bf16/fp16 exact ties among low-probability filler children (torch.topk orders ties arbitrarily, the
     # kernel by index); they never sit on a committed path (checked token by token above)
     assert same / total >= 0.95, f"{total - same}/{total} tree nodes diverge from the oracle under identical ancestors"

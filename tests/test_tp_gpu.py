@@ -1,6 +1,6 @@
-"""Tensor-parallel parity on >= 2 B200s: the target sharded 2-way over NCCL/NVLink (draft head replicated) must emit
-exactly the tokens of the reference (golden vectors), i.e. of the single-GPU engine.  Skipped on a 1-GPU box; run with
-`gpurun --gpus 2 -- python -m pytest tests/test_tp_gpu.py -m gpu`.  Each rank is a separate process with a hard
+"""Tensor-parallel parity on >= 2 H100s: the target sharded 2-way over NCCL/NVLink (draft head replicated) must emit
+exactly the tokens of the reference (golden vectors), i.e. of the single-GPU engine.  Skipped with fewer than 2 GPUs; run
+with `python -m pytest tests/test_tp_gpu.py -m gpu` on a machine with two.  Each rank is a separate process with a hard
 deadline (a rank that dies would otherwise leave its peer blocked in a collective)."""
 import json
 import os

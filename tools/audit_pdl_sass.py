@@ -50,9 +50,6 @@ def audit(target):
             elif not seen_wait:
                 t = re.sub(r"^@!?U?P\d+\s+", "", text)
                 if BAD.match(t) and not t.startswith(("LDC", "LDCU", "LDS", "LDSM", "LDL", "STS", "STL")):
-                    # the GEMM kernels read the TMEM base address back from shared memory through a generic pointer (LD.E)
-                    if t.startswith("LD.E ") and "skinny_gemm" in fn:
-                        continue
                     hits.append(text.strip())
         flush()
     return n_kernels, bad

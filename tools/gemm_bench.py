@@ -1,10 +1,11 @@
-"""Micro-benchmark of the tcgen05/TMA skinny GEMM on the benchmark's projection shapes.
+"""Micro-benchmark of the wgmma/TMA skinny GEMM on the benchmark's projection shapes.
 usage: python tools/gemm_bench.py [graph=1]   (knobs through the EB200_* environment, read once per process)"""
 import ctypes as C
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from bench import measured_peaks  # noqa: E402
 from eagle_b200 import _lib  # noqa: E402
 
 SHAPES = [  # name, epi, M, N, K
@@ -19,7 +20,7 @@ def main():
     global SHAPES
     if len(sys.argv) > 2:  # custom shapes: name:epi:M:N:K,...
         SHAPES = [(f"{a[0]:8s}", int(a[1]), int(a[2]), int(a[3]), int(a[4])) for a in (x.split(":") for x in sys.argv[2].split(","))]
-    peak = 6567.7
+    peak, _ = measured_peaks()  # GB/s: MEASURED_PEAKS.json if present, else the H100 SXM data sheet's 3350
     for name, epi, M, N, K in SHAPES:
         bytes_ = N * K * 2 * (2 if epi == 2 else 1)
         nw = max(2, min(24, int(3e9 // bytes_)))
