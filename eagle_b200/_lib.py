@@ -11,10 +11,10 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libeagle_b200.so")
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 BF16, FP16 = 0, 1
-DT_BF16, DT_FP16, DT_FP32, DT_INT64, DT_BOOL = 0, 1, 2, 3, 4
-FLAG_SIMT_GEMM, FLAG_NO_GRAPH, FLAG_NO_CHAIN = 1, 2, 4
+DT_BF16, DT_FP16, DT_FP32, DT_INT64, DT_BOOL, DT_INT8 = 0, 1, 2, 3, 4, 5
+FLAG_SIMT_GEMM, FLAG_NO_GRAPH, FLAG_NO_CHAIN, FLAG_TARGET_INT8 = 1, 2, 4, 8
 EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU = 0, 1, 2
 
 
@@ -89,6 +89,7 @@ SIGNATURES = {
     "eb200_get_stats": (_I32, [_P, C.POINTER(Stats)]),
     "eb200_reset_stats": (_I32, [_P]),
     "eb200_k_gemm": (_I32, [_I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P]),
+    "eb200_k_gemm_w8": (_I32, [_I32, _I32, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P]),
     "eb200_k_chain_layer": (_I32, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P, _P,
                                     _P, _I32, C.c_float, _P]),
     "eb200_k_chain_gemm": (_I32, [_I32, _I32, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P]),

@@ -11,7 +11,7 @@ from __future__ import annotations
 import glob
 import json
 import os
-from typing import Iterator, Tuple
+from typing import Iterator, Optional, Tuple
 
 import torch
 
@@ -46,6 +46,55 @@ def iter_checkpoint_tensors(directory: str, prefer_bin: bool = False) -> Iterato
     raise FileNotFoundError(f"no *.safetensors or pytorch_model*.bin under {directory}")
 
 
+def target_weights_int8(config: dict, load_in_8bit=False, load_in_4bit=False) -> bool:
+    """Whether the target's decoder projections load as int8 (EaModel `load_in_8bit`).  True for `load_in_8bit=True` on a
+    bf16 / fp16 checkpoint and for a checkpoint transformers saved in bitsandbytes 8-bit format (`quantization_config` with
+    `load_in_8bit: true`), whose stored int8 values are used as they are.  Raises ValueError, before anything is loaded, for
+    what is not supported: 4-bit loading and any other quantization_config (4-bit, fp8, gptq, ...)."""
+    supported = ("supported: load_in_8bit=True (int8 target projections in bitsandbytes' weight format, W8A16 arithmetic) "
+                 "on bf16 / fp16 Llama checkpoints or on transformers' bitsandbytes 8-bit checkpoints")
+    if load_in_4bit:
+        raise ValueError(f"eagle_b200 does not load 4-bit weights (load_in_4bit); {supported}")
+    qc = config.get("quantization_config")
+    if qc:
+        method = qc.get("quant_method", "bitsandbytes")
+        if method == "bitsandbytes" and qc.get("load_in_8bit") and not qc.get("load_in_4bit"):
+            return True
+        raise ValueError(f"unsupported quantization_config (quant_method={method!r}, load_in_4bit={qc.get('load_in_4bit')}); "
+                         f"{supported}")
+    return bool(load_in_8bit)
+
+
+def iter_int8_pairs(directory: str) -> Iterator[Tuple[str, torch.Tensor, Optional[torch.Tensor]]]:
+    """Tensors of a target checkpoint as (name, tensor, SCB): an int8 projection `weight` comes with its fp32 `SCB` row
+    scales, every other tensor with None.  `weight_format` entries (older bitsandbytes serializations) are skipped.  Tensors
+    are streamed; a weight waits only for its own SCB (adjacent in sorted safetensors key order)."""
+    from .quant import is_target_projection
+    weights, scales = {}, {}
+    for k, v in iter_checkpoint_tensors(directory):
+        if k.endswith(".weight_format"):
+            continue
+        if k.endswith(".SCB"):
+            base = k[: -len("SCB")]
+            if base in weights:
+                yield base + "weight", weights.pop(base), v
+            else:
+                scales[base] = v
+        elif k.endswith(".weight") and v.dtype == torch.int8:
+            if not is_target_projection(k):
+                raise ValueError(f"{k}: int8 weights are supported for the target decoder projections only")
+            base = k[: -len("weight")]
+            if base in scales:
+                yield k, v, scales.pop(base)
+            else:
+                weights[base] = v
+        else:
+            yield k, v, None
+    if weights or scales:
+        raise ValueError(f"int8 checkpoint {directory}: unpaired weight / SCB entries "
+                         f"{sorted(list(weights) + list(scales))[:4]}")
+
+
 def save_head_checkpoint(directory: str, head_config: dict, head_sd: dict, as_bin: bool = False):
     """Write a draft-head directory in the reference's format (config.json + weights)."""
     os.makedirs(directory, exist_ok=True)
@@ -60,6 +109,8 @@ def save_head_checkpoint(directory: str, head_config: dict, head_sd: dict, as_bi
 
 
 def save_target_checkpoint(directory: str, target_config: dict, target_sd: dict):
+    """HF Llama directory (config.json + model.safetensors).  A state dict holding int8 `weight` + `SCB` pairs is saved the
+    way transformers saves a bitsandbytes 8-bit model: add `quantization_config` with `load_in_8bit: true` to the config."""
     os.makedirs(directory, exist_ok=True)
     with open(os.path.join(directory, "config.json"), "w") as f:
         json.dump({"architectures": ["LlamaForCausalLM"], "model_type": "llama", **target_config}, f, indent=1)

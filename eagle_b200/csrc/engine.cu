@@ -87,6 +87,21 @@ static int make_tmap(CUtensorMap* m, int dtype, const void* ptr, uint64_t rows, 
                                      (unsigned long long)rows, (unsigned long long)cols, box_rows);
   return 0;
 }
+// row-major [rows][cols] int8 weights of the W8A16 GEMM; box = 128 rows x 64 columns (64 B), unswizzled (the MMA warpgroups read
+// it with generic loads and write the swizzled model-dtype tile themselves)
+static int make_tmap_w8(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols) {
+  TRY(resolve_encode());
+  if (cols % 16) return fail("int8 tensor map: row pitch %llu B is not a multiple of 16", (unsigned long long)cols);
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {cols};
+  cuuint32_t box[2] = {64, 128};
+  cuuint32_t es[2] = {1, 1};
+  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (int8) failed (%d) rows=%llu cols=%llu", (int)r, (unsigned long long)rows,
+                                     (unsigned long long)cols);
+  return 0;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // engine data
@@ -94,8 +109,11 @@ static int make_tmap(CUtensorMap* m, int dtype, const void* ptr, uint64_t rows, 
 struct Linear {
   void* w = nullptr;
   int N = 0, K = 0;
+  int esize = 2;              // bytes per weight: 2 (model dtype) or 1 (int8, EB200_FLAG_TARGET_INT8)
+  float* scale = nullptr;     // int8 only: fp32 scale of each row (SCB)
   CUtensorMap tm;
-  uint64_t loaded_rows = 0;  // bookkeeping for fused / sharded loads
+  uint64_t loaded_rows = 0;   // bookkeeping for fused / sharded loads
+  uint64_t loaded_scales = 0;
 };
 struct ActBuf {  // an activation buffer usable as the X operand of the GEMM (64 rows; 256 where the prompt prefill runs through it)
   void* p = nullptr;
@@ -257,10 +275,12 @@ static int dalloc(eb200_engine* e, void** p, size_t bytes, bool zero = true) {
   if (zero) CK(cudaMemsetAsync(*p, 0, bytes, e->stream));
   return 0;
 }
-static int alloc_linear(eb200_engine* e, Linear& l, int N, int K) {
+static int alloc_linear(eb200_engine* e, Linear& l, int N, int K, bool int8 = false) {
   l.N = N;
   l.K = K;
-  return dalloc(e, &l.w, static_cast<size_t>(N) * K * 2, false);
+  l.esize = int8 ? 1 : 2;
+  if (int8) TRY(dalloc(e, reinterpret_cast<void**>(&l.scale), static_cast<size_t>(N) * 4, false));
+  return dalloc(e, &l.w, static_cast<size_t>(N) * K * l.esize, false);
 }
 static int alloc_act(eb200_engine* e, ActBuf& a, int cols, int rows = 64) {
   a.cols = cols;
@@ -353,11 +373,12 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
     // ---- target weights
     TRY(dalloc(e, &e->t_embed, static_cast<size_t>(e->V) * H * 2, false));
     e->tl.resize(e->L);
+    const bool w8 = (c.flags & EB200_FLAG_TARGET_INT8) != 0;
     for (auto& l : e->tl) {
-      TRY(alloc_linear(e, l.qkv, (e->nh_l + 2 * e->nkv_l) * 128, H));
-      TRY(alloc_linear(e, l.o, H, e->nh_l * 128));
-      TRY(alloc_linear(e, l.gu, 2 * e->I_l, H));
-      TRY(alloc_linear(e, l.down, H, e->I_l));
+      TRY(alloc_linear(e, l.qkv, (e->nh_l + 2 * e->nkv_l) * 128, H, w8));
+      TRY(alloc_linear(e, l.o, H, e->nh_l * 128, w8));
+      TRY(alloc_linear(e, l.gu, 2 * e->I_l, H, w8));
+      TRY(alloc_linear(e, l.down, H, e->I_l, w8));
       TRY(dalloc(e, &l.ln1, H * 2, false));
       TRY(dalloc(e, &l.ln2, H * 2, false));
     }
@@ -563,11 +584,11 @@ extern "C" void eb200_destroy(eb200_engine* e) {
 // ------------------------------------------------------------------------------------------------------------
 // weight loading
 // ------------------------------------------------------------------------------------------------------------
-// copy rows [r0, r0+nr) x cols [c0, c0+nc) of a row-major [R][C] 2-byte source into dst rows [dr0, ...) of pitch nc
-static int copy_block(eb200_engine* e, void* dst, long dst_row0, const void* src, long C, long r0, long nr, long c0, long nc) {
-  const char* s = reinterpret_cast<const char*>(src) + (r0 * C + c0) * 2;
-  char* d = reinterpret_cast<char*>(dst) + dst_row0 * nc * 2;
-  CK(cudaMemcpy2DAsync(d, nc * 2, s, C * 2, nc * 2, nr, cudaMemcpyDefault, e->stream));
+// copy rows [r0, r0+nr) x cols [c0, c0+nc) of a row-major [R][C] source of `es`-byte elements into dst rows [dr0, ...) of pitch nc
+static int copy_block(eb200_engine* e, void* dst, long dst_row0, const void* src, long C, long r0, long nr, long c0, long nc, long es = 2) {
+  const char* s = reinterpret_cast<const char*>(src) + (r0 * C + c0) * es;
+  char* d = reinterpret_cast<char*>(dst) + dst_row0 * nc * es;
+  CK(cudaMemcpy2DAsync(d, nc * es, s, C * es, nc * es, nr, cudaMemcpyDefault, e->stream));
   return 0;
 }
 static bool shape_is(const int64_t* s, int nd, int64_t a, int64_t b = -1) {
@@ -609,54 +630,72 @@ extern "C" int eb200_tp_shard(const char* name, int64_t rows, int64_t cols, int3
 
 // gate_proj (half 0) / up_proj (half 1) rows land interleaved in 64-row groups: source row i of the shard goes to row
 // (i / 64) * 128 + half * 64 + i % 64, so that every 128-row GEMM tile holds the gate AND up rows of the same 64 outputs
-static int copy_interleaved64(eb200_engine* e, void* dst, int half, const void* src, long C, const Shard& sh) {
+// (row scales of int8 weights follow their rows: C = 1, es = 4)
+static int copy_interleaved64(eb200_engine* e, void* dst, int half, const void* src, long C, const Shard& sh, long es = 2) {
   if (sh.nr % 64 || sh.c0 != 0 || sh.nc != C) return fail("gate/up shard must be whole rows in multiples of 64");
-  const char* s = reinterpret_cast<const char*>(src) + sh.r0 * C * 2;
-  char* d = reinterpret_cast<char*>(dst) + static_cast<size_t>(half) * 64 * C * 2;
-  CK(cudaMemcpy2DAsync(d, static_cast<size_t>(128) * C * 2, s, static_cast<size_t>(64) * C * 2, static_cast<size_t>(64) * C * 2, sh.nr / 64,
+  const char* s = reinterpret_cast<const char*>(src) + sh.r0 * C * es;
+  char* d = reinterpret_cast<char*>(dst) + static_cast<size_t>(half) * 64 * C * es;
+  CK(cudaMemcpy2DAsync(d, static_cast<size_t>(128) * C * es, s, static_cast<size_t>(64) * C * es, static_cast<size_t>(64) * C * es, sh.nr / 64,
                        cudaMemcpyDefault, e->stream));
   return 0;
+}
+
+static bool ends_with(const std::string& s, const char* suf) {
+  const size_t n = strlen(suf);
+  return s.size() >= n && s.compare(s.size() - n, n, suf) == 0;
+}
+// the seven decoder-layer projections: weight "<proj>.weight"; int8 row scales "<proj>.SCB" (EB200_FLAG_TARGET_INT8)
+static const char* const kProjNames[7] = {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj",
+                                          "mlp.gate_proj",    "mlp.up_proj",      "mlp.down_proj"};
+static int proj_index(const std::string& sub, bool* scb) {
+  for (int i = 0; i < 7; ++i) {
+    const std::string p(kProjNames[i]);
+    if (sub == p + ".weight" || sub == p + ".SCB") {
+      *scb = sub == p + ".SCB";
+      return i;
+    }
+  }
+  return -1;
 }
 
 static int load_layer_tensor(eb200_engine* e, Layer& l, const std::string& sub, const void* data, const int64_t* shape,
                              int nd, bool is_target, int Hin_qkv, int Hm, int nh_full, int nkv_full, int I_full) {
   const int tp = is_target ? e->c.tp_size : 1, rk = is_target ? e->c.tp_rank : 0;
   const int nh_l = nh_full / tp, nkv_l = nkv_full / tp;
-  if (sub == "self_attn.q_proj.weight") {
-    if (!shape_is(shape, nd, nh_full * 128, Hin_qkv)) return fail("q_proj shape mismatch");
-    const Shard sh = shard_of(sub, nh_full * 128, Hin_qkv, rk, tp);
-    TRY(copy_block(e, l.qkv.w, 0, data, Hin_qkv, sh.r0, sh.nr, sh.c0, sh.nc));
-    l.qkv.loaded_rows |= 1;
-  } else if (sub == "self_attn.k_proj.weight") {
-    if (!shape_is(shape, nd, nkv_full * 128, Hin_qkv)) return fail("k_proj shape mismatch");
-    const Shard sh = shard_of(sub, nkv_full * 128, Hin_qkv, rk, tp);
-    TRY(copy_block(e, l.qkv.w, nh_l * 128, data, Hin_qkv, sh.r0, sh.nr, sh.c0, sh.nc));
-    l.qkv.loaded_rows |= 2;
-  } else if (sub == "self_attn.v_proj.weight") {
-    if (!shape_is(shape, nd, nkv_full * 128, Hin_qkv)) return fail("v_proj shape mismatch");
-    const Shard sh = shard_of(sub, nkv_full * 128, Hin_qkv, rk, tp);
-    TRY(copy_block(e, l.qkv.w, (nh_l + nkv_l) * 128, data, Hin_qkv, sh.r0, sh.nr, sh.c0, sh.nc));
-    l.qkv.loaded_rows |= 4;
-  } else if (sub == "self_attn.o_proj.weight") {
-    if (!shape_is(shape, nd, Hm, nh_full * 128)) return fail("o_proj shape mismatch");
-    const Shard sh = shard_of(sub, Hm, nh_full * 128, rk, tp);
-    TRY(copy_block(e, l.o.w, 0, data, nh_full * 128, sh.r0, sh.nr, sh.c0, sh.nc));
-    l.o.loaded_rows = 1;
-  } else if (sub == "mlp.gate_proj.weight") {
-    if (!shape_is(shape, nd, I_full, Hm)) return fail("gate_proj shape mismatch");
-    const Shard sh = shard_of(sub, I_full, Hm, rk, tp);
-    TRY(copy_interleaved64(e, l.gu.w, 0, data, Hm, sh));
-    l.gu.loaded_rows |= 1;
-  } else if (sub == "mlp.up_proj.weight") {
-    if (!shape_is(shape, nd, I_full, Hm)) return fail("up_proj shape mismatch");
-    const Shard sh = shard_of(sub, I_full, Hm, rk, tp);
-    TRY(copy_interleaved64(e, l.gu.w, 1, data, Hm, sh));
-    l.gu.loaded_rows |= 2;
-  } else if (sub == "mlp.down_proj.weight") {
-    if (!shape_is(shape, nd, Hm, I_full)) return fail("down_proj shape mismatch");
-    const Shard sh = shard_of(sub, Hm, I_full, rk, tp);
-    TRY(copy_block(e, l.down.w, 0, data, I_full, sh.r0, sh.nr, sh.c0, sh.nc));
-    l.down.loaded_rows = 1;
+  bool scb = false;
+  const int pi = proj_index(sub, &scb);
+  if (pi >= 0) {
+    // destination matrix, full [rows, cols] of the checkpoint tensor, first destination row, gate/up half, loaded bit
+    struct Slot {
+      Linear* lin;
+      long rows, cols, row0;
+      int half, bit;
+    };
+    const Slot slots[7] = {{&l.qkv, nh_full * 128L, Hin_qkv, 0, -1, 1},
+                           {&l.qkv, nkv_full * 128L, Hin_qkv, nh_l * 128L, -1, 2},
+                           {&l.qkv, nkv_full * 128L, Hin_qkv, (nh_l + nkv_l) * 128L, -1, 4},
+                           {&l.o, Hm, nh_full * 128L, 0, -1, 1},
+                           {&l.gu, I_full, Hm, 0, 0, 1},
+                           {&l.gu, I_full, Hm, 0, 1, 2},
+                           {&l.down, Hm, I_full, 0, -1, 1}};
+    const Slot& sl = slots[pi];
+    const char* short_name = strchr(kProjNames[pi], '.') + 1;
+    const std::string wname = std::string(kProjNames[pi]) + ".weight";
+    const Shard sh = shard_of(wname, sl.rows, sl.cols, rk, tp);
+    Linear& L = *sl.lin;
+    if (!scb) {
+      if (!shape_is(shape, nd, sl.rows, sl.cols)) return fail("%s shape mismatch", short_name);
+      if (sl.half >= 0) TRY(copy_interleaved64(e, L.w, sl.half, data, sl.cols, sh, L.esize));
+      else TRY(copy_block(e, L.w, sl.row0, data, sl.cols, sh.r0, sh.nr, sh.c0, sh.nc, L.esize));
+      L.loaded_rows |= sl.bit;
+    } else {
+      if (!L.scale) return fail("%s.SCB: row scales belong to int8 projections (EB200_FLAG_TARGET_INT8)", short_name);
+      if (!shape_is(shape, nd, sl.rows)) return fail("%s.SCB shape mismatch (want [%ld] fp32)", short_name, sl.rows);
+      const Shard rs{sh.r0, sh.nr, 0, 1};  // the scales shard with their rows
+      if (sl.half >= 0) TRY(copy_interleaved64(e, L.scale, sl.half, data, 1, rs, 4));
+      else TRY(copy_block(e, L.scale, sl.row0, data, 1, rs.r0, rs.nr, 0, 1, 4));
+      L.loaded_scales |= sl.bit;
+    }
   } else if (sub == "input_layernorm.weight") {
     if (!l.ln1) return 0;  // EAGLE-1 layer 0 has no input norm (cnets1.py:399-401): ignore like strict=False
     if (!shape_is(shape, nd, Hm)) return fail("input_layernorm shape mismatch");
@@ -682,10 +721,25 @@ extern "C" int eb200_load_tensor(eb200_engine* e, const char* name_c, const void
   std::string name(name_c);
   const bool is_head = name.rfind("head.", 0) == 0;
   const bool want_model_dtype = !(name == "head.d2t" || name == "head.t2d");
-  if (want_model_dtype && dtype != e->dtype)
+  const eb200_config& c = e->c;
+  // int8 target projections: "<proj>.weight" int8 + "<proj>.SCB" fp32, only on an engine created with EB200_FLAG_TARGET_INT8
+  bool scb = false;
+  const bool target_proj = !is_head && name.rfind("model.layers.", 0) == 0 && name.find('.', strlen("model.layers.")) != std::string::npos &&
+                           proj_index(name.substr(name.find('.', strlen("model.layers.")) + 1), &scb) >= 0;
+  const bool w8 = (c.flags & EB200_FLAG_TARGET_INT8) != 0;
+  if (dtype == EB200_DT_INT8 || ends_with(name, ".SCB")) {
+    if (!target_proj)
+      return fail("tensor '%s': int8 weights and SCB row scales are accepted only for the target decoder projections "
+                  "(q/k/v/o/gate/up/down_proj); embeddings, norms, lm_head and the draft head stay in the model dtype", name_c);
+    if (!w8) return fail("tensor '%s': int8 data for an engine created without EB200_FLAG_TARGET_INT8 (load_in_8bit)", name_c);
+    if (scb && dtype != EB200_DT_FP32) return fail("tensor '%s': SCB row scales must be fp32", name_c);
+  } else if (w8 && target_proj) {
+    return fail("tensor '%s': this engine stores the target projections in int8 (EB200_FLAG_TARGET_INT8): pass the int8 weight and "
+                "its fp32 SCB row scales (eagle_b200.quant.quantize_int8_rowwise)", name_c);
+  } else if (want_model_dtype && dtype != e->dtype) {
     return fail("tensor '%s': dtype %d does not match the engine's model dtype %d (cast it like `.to(base_model.dtype)`, ea_model.py:77)",
                 name_c, dtype, e->dtype);
-  const eb200_config& c = e->c;
+  }
   if (!is_head) {
     if (name == "model.embed_tokens.weight") {
       if (!shape_is(shape, ndim, e->V, e->H)) return fail("embed_tokens shape mismatch");
@@ -784,12 +838,29 @@ extern "C" int eb200_set_rope_table(eb200_engine* e, int32_t which, const void* 
 
 static int finalize_linear(eb200_engine* e, Linear& l, const char* what, uint64_t need) {
   if (l.loaded_rows != need) return fail("weights missing for %s", what);
+  if (l.scale) {
+    if (l.loaded_scales != need) return fail("SCB row scales missing for %s (int8 weights need their fp32 row scales)", what);
+    return make_tmap_w8(&l.tm, l.w, l.N, l.K);
+  }
   return make_tmap(&l.tm, e->dtype, l.w, l.N, l.K, 128);
 }
 
+static int gemm_mode();
 extern "C" int eb200_finalize(eb200_engine* e) {
   if (!e) return fail("eb200_finalize: null engine");
   CK(cudaSetDevice(e->c.device));
+  if (e->c.flags & EB200_FLAG_TARGET_INT8) {
+    // the W8A16 GEMM exists as the cluster split-K kernel of one GPU only
+    const char* what = nullptr;
+    const char* chain = getenv("EB200_CHAIN");
+    if (e->c.tp_size > 1) what = "tensor parallelism (tp_size > 1)";
+    else if (e->c.flags & EB200_FLAG_SIMT_GEMM) what = "EB200_FLAG_SIMT_GEMM";
+    else if (chain && atoi(chain) == 1) what = "EB200_CHAIN=1 (persistent layer-segment launches)";
+    else if (gemm_mode() == 0) what = "EB200_GEMM_MODE=streamk";
+    if (what)
+      return fail("int8 target weights (EB200_FLAG_TARGET_INT8) are not supported with %s; they run on one GPU with the default "
+                  "cluster split-K GEMM", what);
+  }
   char nm[128];
   if (!e->t_embed_loaded || !e->t_norm_loaded) return fail("target embed/norm weights missing");
   for (int i = 0; i < e->L; ++i) {
@@ -989,7 +1060,9 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
   p.counters = e->counters;
   p.splitk = pick_splitk(p.N, p.K, cx.mpad, g.epi, e->ws_bytes);
   if ((p.N + 127) / 128 > 8192) return fail("too many n tiles");
-  const double bytes = static_cast<double>(p.N) * p.K * 2 * (g.epi == EPI_SWIGLU ? 2 : 1);
+  p.w_scale = g.W->scale;
+  // algorithmic weight bytes: int8 weights stream N*K bytes plus the N fp32 row scales
+  const double bytes = p.w_scale ? static_cast<double>(p.N) * p.K + 4.0 * p.N : static_cast<double>(p.N) * p.K * 2 * (g.epi == EPI_SWIGLU ? 2 : 1);
   const char* kname = g.epi == EPI_STORE ? "gemm_store" : g.epi == EPI_RESIDUAL ? "gemm_residual" :
                       (g.epi == EPI_SWIGLU || g.epi == EPI_SWIGLU_IL) ? "gemm_swiglu" : "gemm_qkv_rope";
   {
@@ -998,7 +1071,11 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
     if (skip_kernel(kname) || skip_kernel(kk)) return 0;
   }
   ProfScope ps(e, 0, bytes, kname);
-  if (e->c.flags & EB200_FLAG_SIMT_GEMM) {
+  if (p.w_scale) {
+    if (cx.mpad == 256 && g.X->rows < 256) return fail("256-row GEMM on a 64-row activation buffer");
+    CKL(launch_gemm_w8(e->dtype, cx.mpad, g.epi, &g.W->tm, cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256), p,
+                       e->stream));
+  } else if (e->c.flags & EB200_FLAG_SIMT_GEMM) {
     const size_t per_split = static_cast<size_t>(g.epi == EPI_SWIGLU ? 2 : 1) * cx.mpad * ((p.N + 127) / 128) * 128 * 4;
     while (p.splitk > 1 && per_split * p.splitk > e->ws_bytes) --p.splitk;
     CKL(launch_gemm_simt(e->dtype, cx.mpad, g.epi, g.W->w, g.W2 ? g.W2->w : nullptr, g.X->p, g.X->cols, p, e->stream));
@@ -1240,7 +1317,7 @@ static int attention(eb200_engine* e, const RowCtx& cx, const void* q, void* kc,
     const Linear* nx[2] = {next0, next1};
     for (int r = 0; r < 2; ++r) {
       if (!nx[r] || left <= 0) continue;
-      const long bytes = std::min<long>(left, static_cast<long>(nx[r]->N) * nx[r]->K * 2);
+      const long bytes = std::min<long>(left, static_cast<long>(nx[r]->N) * nx[r]->K * nx[r]->esize);
       a.pf_ptr[r] = nx[r]->w;
       a.pf_bytes[r] = static_cast<unsigned long long>(bytes);
       left -= bytes;
@@ -2581,6 +2658,39 @@ extern "C" int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const
       CKL(launch_gemm_streamk(dtype, mpad, epilogue, &tw, W2 ? &tw2 : nullptr, &tx, p, skws, counters, s));
     }
   }
+  CK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+extern "C" int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, const void* scb, const void* X, void* out, const void* res,
+                               const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream) {
+  if (M < 1 || M > 64 || (epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !scb || splitk < 1 ||
+      splitk > 8)
+    return fail("eb200_k_gemm_w8: bad arguments");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const int mpad = M <= 16 ? 16 : 64;
+  const int n_out = N;  // EPI_SWIGLU_IL: Wq is the [2N, K] interleaved gate/up matrix, out is [M, N]
+  if (epilogue == EPI_SWIGLU_IL) {
+    if (N % 64) return fail("eb200_k_gemm_w8: interleaved SwiGLU needs N % 64 == 0");
+    N *= 2;
+  }
+  GemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.N = N;
+  p.K = K;
+  p.m_rows = M;
+  p.m_idx = -1;
+  p.splitk = splitk;
+  p.out = out;
+  p.ld_out = n_out;
+  p.res = res;
+  p.ld_res = n_out;
+  p.bias = bias;
+  p.w_scale = reinterpret_cast<const float*>(scb);
+  CUtensorMap tw, tx;
+  TRY(make_tmap_w8(&tw, Wq, N, K));
+  TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
+  CKL(launch_gemm_w8(dtype, mpad, epilogue, &tw, &tx, p, s));
   CK(cudaStreamSynchronize(s));
   return 0;
 }

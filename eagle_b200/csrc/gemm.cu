@@ -43,15 +43,67 @@ static int smem_budget(int total_ctas) {
   }
   return (total_ctas <= device_sm_count() ? big_kb : small_kb) * 1024;
 }
-static int stage_count_for(int mpad, int epi, int total_ctas) {
+static int stage_count_for(int mpad, int epi, int total_ctas, bool w8 = false) {
   // 256 activation rows (prefill): a stage is 48 KB and the cluster reduction parks 128 KB of partials, so always one CTA per SM
   const int budget = mpad >= 256 ? 200 * 1024 : smem_budget(total_ctas);
-  int s = (budget - kCtrlBytes - 1024) / stage_bytes(mpad, epi);
+  int s = w8 ? (budget - kCtrlBytes - 1024 - kW8DqBytes) / stage_bytes_w8(mpad) : (budget - kCtrlBytes - 1024) / stage_bytes(mpad, epi);
   if (s > kMaxStages) s = kMaxStages;
   if (s < 2) s = 2;
   return s;
 }
 int gemm_stage_count(int mpad, int epi) { return stage_count_for(mpad, epi, 1 << 30); }
+
+// ------------------------------------------------------------------------------------------------------------
+// W8A16 dequantization: one warpgroup turns its 64 int8 weight rows of a stage (row-major, 64 B per row) into the model-dtype
+// K-major SWIZZLE_128B layout wgmma reads (16-byte chunk c of row r at r * 128 + ((c ^ (r & 7)) * 16)).  Thread t handles the
+// 16-element chunks t and t + 128, i.e. rows t / 4 and 32 + t / 4; sc[j] is the scale of its row j.  Arithmetic: transformers'
+// dequantization T((q * SCB) * kInv127), two fp32 roundings and one cast, no FMA contraction.
+// ------------------------------------------------------------------------------------------------------------
+// exact int8 -> fp32 of byte b of w without a conversion instruction: with u = byte ^ 0x80 in [0, 255], the bit pattern
+// 0x4B0000uu is the fp32 value 2^23 + u, and subtracting 2^23 + 128 leaves the signed byte exactly
+__device__ __forceinline__ float i8_to_f32(uint32_t w_xor80, int b) {
+  return __fsub_rn(__uint_as_float(__byte_perm(w_xor80, 0x4B000000u, 0x7540u + b)), 8388736.0f);
+}
+template <typename T> __device__ __forceinline__ uint32_t pack2_rn(float lo, float hi);
+template <> __device__ __forceinline__ uint32_t pack2_rn<__nv_bfloat16>(float lo, float hi) {
+  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&v);
+}
+template <> __device__ __forceinline__ uint32_t pack2_rn<__half>(float lo, float hi) {
+  const __half2 v = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&v);
+}
+template <typename T> __device__ __forceinline__ uint32_t dq_pack2(uint32_t w_xor80, int b, float s) {
+  const float lo = __fmul_rn(__fmul_rn(i8_to_f32(w_xor80, b), s), kInv127);
+  const float hi = __fmul_rn(__fmul_rn(i8_to_f32(w_xor80, b + 1), s), kInv127);
+  return pack2_rn<T>(lo, hi);
+}
+template <typename T> __device__ __forceinline__ void dequant_w8_rows(uint32_t src, uint32_t dst, const float (&sc)[2]) {
+  const int t = threadIdx.x & 127;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int r = 32 * j + (t >> 2), c = t & 3;
+    uint32_t w[4];
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "r"(src + r * 64 + c * 16));
+    uint32_t o[8];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      o[2 * i] = dq_pack2<T>(w[i] ^ 0x80808080u, 0, sc[j]);
+      o[2 * i + 1] = dq_pack2<T>(w[i] ^ 0x80808080u, 2, sc[j]);
+    }
+    const uint32_t row = dst + r * 128;
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(row + (((2 * c) ^ (r & 7)) * 16)), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3])
+                 : "memory");
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(row + (((2 * c + 1) ^ (r & 7)) * 16)), "r"(o[4]), "r"(o[5]), "r"(o[6]),
+                 "r"(o[7])
+                 : "memory");
+  }
+}
+__device__ __forceinline__ float ld_global_f32(const float* p) {
+  float v;
+  asm volatile("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
+  return v;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // wgmma + TMA kernel
@@ -63,18 +115,25 @@ int gemm_stage_count(int mpad, int epi) { return stage_count_for(mpad, epi, 1 <<
 // XMC: the two CTAs of neighbouring n-tiles (cluster dimension x = 2) stream the SAME activation k-range; each loads one half of
 // every X tile (32 rows) and TMA-multicasts it into both CTAs' rings, so the L2 -> shared-memory ingress of an SM carries half
 // the X bytes.
-template <typename T, int MPAD, int EPI, bool XMC>
+// W8: tmW streams int8 weight tiles; the MMA warpgroups dequantize every stage into one model-dtype tile (an 8 KB half per
+// warpgroup) and run the same k16 MMAs on it, so the accumulators equal those of the kernel on the dequantized W.  Each k-block's
+// MMAs retire before the next dequantization (wgmma_wait<0>): ptxas serialises every wgmma of a kernel whose MMAs stay in flight
+// across the conversion code.  The other warpgroup and the second resident CTA keep the tensor pipe and the TMA ring busy meanwhile.
+template <typename T, int MPAD, int EPI, bool XMC, bool W8>
 __global__ void __launch_bounds__(kGemmThreads, (MPAD >= 256 ? 1 : 2))
 skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmW2,
                   const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXh, const GemmParams p, const int stages) {
   constexpr bool kDual = (EPI == EPI_SWIGLU);
   static_assert(!XMC || (MPAD == 64 && !kDual), "X multicast: 64-row tiles, single accumulator");
-  constexpr int kStageBytes = stage_bytes(MPAD, EPI);
+  static_assert(!W8 || (!XMC && !kDual), "W8A16: single weight stream, no X multicast");
+  constexpr int kWBytes = W8 ? kW8TileBytes : kWTileBytes;  // weight bytes of one stage (per weight matrix)
+  constexpr int kStageBytes = W8 ? stage_bytes_w8(MPAD) : stage_bytes(MPAD, EPI);
   constexpr int kPartBytes = acc_tile_bytes(MPAD, EPI);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* ctrl = smem + stages * kStageBytes;
+  uint8_t* wdq = smem + stages * kStageBytes;  // W8: the dequantized weight tile
+  uint8_t* ctrl = wdq + (W8 ? kW8DqBytes : 0);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);
   uint64_t* empty_bar = full_bar + kMaxStages;
 
@@ -121,7 +180,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
       }
       pdl_wait();
       auto load_x = [&](int stage, int kb) {
-        uint8_t* xdst = smem + stage * kStageBytes + kWTileBytes * (kDual ? 2 : 1);
+        uint8_t* xdst = smem + stage * kStageBytes + kWBytes * (kDual ? 2 : 1);
         if constexpr (XMC) {
           tma_load_2d_multicast(xdst + xpar * (32 * kBlockK * 2), &tmXh, &full_bar[stage], kb * kBlockK, static_cast<int>(xpar) * 32, pair_mask,
                                 kEvictLast);
@@ -159,20 +218,41 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
         if constexpr (XMC) mbar_arrive_cluster(&empty_bar[st], crank ^ 1u);  // the neighbour's half of this slot is consumed too
       }
     };
+    float sc[2] = {0.f, 0.f};
+    if constexpr (W8) {
+      pdl_wait();  // the row scales are read with generic loads, which may not precede the dependency wait
+      const int t = threadIdx.x & 127;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int n = n_tile * kBlockN + wg * 64 + 32 * j + (t >> 2);  // the rows dequant_w8_rows gives this thread
+        if (n < p.N) sc[j] = ld_global_f32(p.w_scale + n);
+      }
+    }
     int s = 0, prev = -1;
     uint32_t ph = 0;
     for (int kb = kb_begin; kb < kb_end; ++kb) {
       mbar_wait_mma(&full_bar[s], ph);
       const uint32_t st = smem_u32(smem + s * kStageBytes);
-      const uint32_t a_addr = st + wg * (kWTileBytes / 2);  // 64 weight rows = 8 KB = eight whole swizzle atoms
-      const uint64_t b_desc = make_kmajor_sw128_desc(st + kWTileBytes * (kDual ? 2 : 1));
+      uint32_t a_addr = st + wg * (kWTileBytes / 2);  // 64 weight rows = 8 KB = eight whole swizzle atoms
+      if constexpr (W8) {
+        a_addr = smem_u32(wdq) + wg * (kWTileBytes / 2);
+        dequant_w8_rows<T>(st + wg * (kW8TileBytes / 2), a_addr, sc);
+        fence_proxy_async();  // generic-proxy stores -> async-proxy (wgmma) reads
+        asm volatile("bar.sync %0, 128;" ::"r"(3 + wg) : "memory");
+      }
+      const uint64_t b_desc = make_kmajor_sw128_desc(st + kWBytes * (kDual ? 2 : 1));
       wgmma_fence();
       wgmma_kblock<T, MPAD>(acc, make_kmajor_sw128_desc(a_addr), b_desc);
       if constexpr (kDual) wgmma_kblock<T, MPAD>(acc2, make_kmajor_sw128_desc(a_addr + kWTileBytes), b_desc);
       wgmma_commit();
-      wgmma_wait<1>();  // the previous k-block's MMAs have retired: its slot can be refilled
-      if (prev >= 0) release(prev);
-      prev = s;
+      if constexpr (W8) {
+        wgmma_wait<0>();  // this k-block's MMAs have retired: its slot and the dequantized tile can be rewritten
+        release(s);
+      } else {
+        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its slot can be refilled
+        if (prev >= 0) release(prev);
+        prev = s;
+      }
       if (++s == stages) {
         s = 0;
         ph ^= 1;
@@ -342,7 +422,7 @@ static bool xmc_enabled() {
   }
   return v == 1;
 }
-template <typename T, int MPAD, int EPI, bool XMC>
+template <typename T, int MPAD, int EPI, bool XMC, bool W8 = false>
 static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
                         cudaStream_t s);
 template <typename T, int MPAD, int EPI>
@@ -354,16 +434,17 @@ static int launch_one(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUt
   }
   return launch_one_x<T, MPAD, EPI, false>(tmW, tmW2, tmX, tmX, p, s);
 }
-template <typename T, int MPAD, int EPI, bool XMC>
+template <typename T, int MPAD, int EPI, bool XMC, bool W8>
 static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
                         cudaStream_t s) {
-  auto kern = skinny_gemm_wgmma<T, MPAD, EPI, XMC>;
+  auto kern = skinny_gemm_wgmma<T, MPAD, EPI, XMC, W8>;
   dim3 grid((p.N + kBlockN - 1) / kBlockN, p.splitk);
-  const int stages = stage_count_for(MPAD, EPI, static_cast<int>(grid.x * grid.y));
-  const int smem = stages * stage_bytes(MPAD, EPI) + kCtrlBytes + 1024;
+  const int stages = stage_count_for(MPAD, EPI, static_cast<int>(grid.x * grid.y), W8);
+  const int sbytes = W8 ? stage_bytes_w8(MPAD) : stage_bytes(MPAD, EPI);
+  const int smem = stages * sbytes + (W8 ? kW8DqBytes : 0) + kCtrlBytes + 1024;
   if (p.splitk > 8) return static_cast<int>(cudaErrorInvalidValue);  // portable cluster size
   // the accumulators are parked as (1|2) x MPAD x 128 fp32 partials (+ a 4 KB exchange strip) in the stage memory
-  if (stages * stage_bytes(MPAD, EPI) < acc_tile_bytes(MPAD, EPI) + 4096)
+  if (stages * sbytes < acc_tile_bytes(MPAD, EPI) + 4096)
     return static_cast<int>(cudaErrorInvalidValue);
   static bool configured_dev[64] = {};  // per device (the attribute is per device) and per instantiation
   const int cur_dev = current_device_index();
@@ -419,6 +500,39 @@ int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUte
     if (mpad == 16) return launch_epi<__half, 16>(epi, tmW, tmW2, tmX, p, s);
     if (mpad == 64) return launch_epi<__half, 64>(epi, tmW, tmW2, tmX, p, s, tmXh);
     if (mpad == 256) return launch_epi256<__half>(epi, tmW, tmX, p, s);
+  }
+  return static_cast<int>(cudaErrorInvalidValue);
+}
+
+// W8A16: the epilogues of the target's decoder layer (+ EPI_STORE for mpad 16 / 64)
+template <typename T, int MPAD>
+static int launch_w8_epi(int epi, const CUtensorMap* w, const CUtensorMap* x, const GemmParams& p, cudaStream_t s) {
+  switch (epi) {
+    case EPI_STORE:
+      if constexpr (MPAD < 256) return launch_one_x<T, MPAD, EPI_STORE, false, true>(w, nullptr, x, x, p, s);
+      break;
+    case EPI_RESIDUAL: return launch_one_x<T, MPAD, EPI_RESIDUAL, false, true>(w, nullptr, x, x, p, s);
+    case EPI_QKV_ROPE: return launch_one_x<T, MPAD, EPI_QKV_ROPE, false, true>(w, nullptr, x, x, p, s);
+    case EPI_SWIGLU_IL: return launch_one_x<T, MPAD, EPI_SWIGLU_IL, false, true>(w, nullptr, x, x, p, s);
+  }
+  return static_cast<int>(cudaErrorInvalidValue);
+}
+
+int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmX, const GemmParams& p_in, cudaStream_t s) {
+  GemmParams p = p_in;
+  if (p.splitk < 1 || p.m_rows > mpad || !p.w_scale) return static_cast<int>(cudaErrorInvalidValue);
+  if (epi == EPI_SWIGLU_IL) {
+    p.silu_lut = silu_lut(dtype, s);
+    if (!p.silu_lut) return static_cast<int>(cudaErrorNotReady);
+  }
+  if (dtype == DT_BF16) {
+    if (mpad == 16) return launch_w8_epi<__nv_bfloat16, 16>(epi, tmW, tmX, p, s);
+    if (mpad == 64) return launch_w8_epi<__nv_bfloat16, 64>(epi, tmW, tmX, p, s);
+    if (mpad == 256) return launch_w8_epi<__nv_bfloat16, 256>(epi, tmW, tmX, p, s);
+  } else if (dtype == DT_FP16) {
+    if (mpad == 16) return launch_w8_epi<__half, 16>(epi, tmW, tmX, p, s);
+    if (mpad == 64) return launch_w8_epi<__half, 64>(epi, tmW, tmX, p, s);
+    if (mpad == 256) return launch_w8_epi<__half, 256>(epi, tmW, tmX, p, s);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }

@@ -20,6 +20,13 @@ __host__ __device__ constexpr int stage_bytes(int mpad, int epi) {
 }
 // fp32 accumulator tile(s) of one CTA staged in shared memory: [acc][MPAD][128]
 __host__ __device__ constexpr int acc_tile_bytes(int mpad, int epi) { return (epi == EPI_SWIGLU ? 2 : 1) * mpad * kBlockN * 4; }
+// W8A16 (int8 weights + one fp32 scale per row): a stage holds the int8 weight tile (128 rows x 64 bytes, unswizzled) and the
+// X tile; the MMA warpgroups dequantize each stage into the model-dtype SWIZZLE_128B tile that follows the ring
+constexpr int kW8TileBytes = kBlockN * kBlockK;
+constexpr int kW8DqBytes = kWTileBytes;
+__host__ __device__ constexpr int stage_bytes_w8(int mpad) { return kW8TileBytes + x_tile_bytes(mpad); }
+// transformers' bnb 8-bit dequantization factor (integrations/bitsandbytes.py), as the fp32 value torch multiplies by
+constexpr float kInv127 = 7.874015718698502e-3f;
 
 // number of SMs of the current device (the grids are sized to fill it)
 inline int device_sm_count() {

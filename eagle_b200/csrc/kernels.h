@@ -81,6 +81,8 @@ struct GemmParams {
   const int* pos_arr;
   int pos_mstride;
   DynInt kv_base;        // K/V rows are appended at kv_base + m
+  // launch_gemm_w8: fp32 scale of each int8 weight row [N] (bitsandbytes' SCB, the row absmax)
+  const float* w_scale;
 };
 
 // Returns cudaError_t-compatible int (0 = ok).  mpad in {16, 64}.  tm* are HOST pointers to encoded maps.
@@ -88,6 +90,11 @@ struct GemmParams {
 // in a cluster share every X tile, each CTA loads half of it)
 int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX,
                 const GemmParams& p, cudaStream_t s, const CUtensorMap* tmXh = nullptr);
+// W8A16 form of launch_gemm: tmW maps an int8 [N][K] weight (make_tmap_w8 layout: box 128 rows x 64 bytes, no swizzle) and
+// p.w_scale its row scales.  The kernel forms W' = T((q * scale) * kInv127) in shared memory and runs the same wgmma sequence and
+// epilogue as launch_gemm, so the result is bit-identical to launch_gemm on W'.  mpad 16 / 64: EPI_STORE, EPI_RESIDUAL,
+// EPI_QKV_ROPE, EPI_SWIGLU_IL; mpad 256: the last three.
+int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmX, const GemmParams& p, cudaStream_t s);
 // bring-up / debugging aid: same epilogues, plain FMA main loop, no TMA/wgmma.  W/W2/X are raw pointers.
 int launch_gemm_simt(int dtype, int mpad, int epi, const void* W, const void* W2, const void* X, long ldx,
                      const GemmParams& p, cudaStream_t s);

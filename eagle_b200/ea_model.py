@@ -20,9 +20,10 @@ from typing import Dict, Iterator, Optional
 import torch
 
 from . import _lib
+from .quant import is_target_projection, quantize_int8_rowwise
 
 _TORCH2ENGINE = {torch.bfloat16: _lib.DT_BF16, torch.float16: _lib.DT_FP16, torch.float32: _lib.DT_FP32,
-                 torch.int64: _lib.DT_INT64, torch.bool: _lib.DT_BOOL}
+                 torch.int64: _lib.DT_INT64, torch.bool: _lib.DT_BOOL, torch.int8: _lib.DT_INT8}
 
 
 def _llama3_inv_freq(inv_freq: torch.Tensor, rs: dict, max_position_embeddings: int) -> torch.Tensor:
@@ -131,7 +132,7 @@ class EaModel(torch.nn.Module):
     def __init__(self, target_config: dict, head_config: dict, use_eagle3: bool = True, total_token: int = 60,
                  depth: int = 7, top_k: int = 10, threshold: float = 1.0, torch_dtype: torch.dtype = torch.bfloat16,
                  device: int = 0, max_length: int = 2048, tokenizer=None, flags: int = 0, tp_rank: int = 0,
-                 tp_size: int = 1, tree_choices=None):
+                 tp_size: int = 1, tree_choices=None, load_in_8bit: bool = False):
         super().__init__()
         self.training = False
         self.lib = _lib.load()
@@ -153,6 +154,10 @@ class EaModel(torch.nn.Module):
         self.tokenizer = tokenizer
         self.threshold = threshold  # stored and never read, like the reference (cnets.py:524)
         self.max_length = int(max_length)
+        # int8 target projections (eagle_b200.quant): bitsandbytes' weight format, exact W8A16 arithmetic
+        self.load_in_8bit = bool(load_in_8bit)
+        if self.load_in_8bit:
+            flags |= _lib.FLAG_TARGET_INT8
         # attributes callers touch (ea_model.py:168; evaluation scripts)
         self.ea_layer = SimpleNamespace(total_tokens=total_token - 1, depth=depth, top_k=top_k)
         self.base_model = SimpleNamespace(config=self.config, dtype=torch_dtype, device=torch.device("cuda", int(device)))
@@ -202,7 +207,7 @@ class EaModel(torch.nn.Module):
     # weights
     # ---------------------------------------------------------------------------------------------
     def _load(self, name: str, t: torch.Tensor):
-        if t.dtype.is_floating_point and t.dtype != self.dtype:
+        if t.dtype.is_floating_point and t.dtype != self.dtype and not name.endswith(".SCB"):
             t = t.to(self.dtype)  # `.to(base_model.dtype)` (ea_model.py:77)
         t = t.contiguous()
         if t.is_cuda:
@@ -211,11 +216,23 @@ class EaModel(torch.nn.Module):
         shape = (C.c_int64 * t.dim())(*t.shape)
         _lib.check(self.lib.eb200_load_tensor(self._h, name.encode(), t.data_ptr(), shape, t.dim(), _TORCH2ENGINE[t.dtype]))
 
+    def _load_target(self, name: str, t: torch.Tensor):
+        """One target tensor; with load_in_8bit a model-dtype projection weight is quantized here (eagle_b200.quant), one tensor
+        at a time, and goes in as its int8 weight + SCB pair."""
+        if self.load_in_8bit and t.dtype.is_floating_point and name.endswith(".weight") and is_target_projection(name):
+            q, scb = quantize_int8_rowwise(t.to(self.dtype))
+            self._load(name, q)
+            self._load(name[: -len("weight")] + "SCB", scb)
+        else:
+            self._load(name, t)
+
     def load_target_state_dict(self, sd: Dict[str, torch.Tensor]):
+        """HF target keys.  With load_in_8bit the projections may be model-dtype weights (quantized while loading) or int8
+        `weight` + fp32 `SCB` pairs (bitsandbytes' serialization); `weight_format` entries are ignored."""
         for k, v in sd.items():
-            if "rotary_emb" in k:
+            if "rotary_emb" in k or k.endswith(".weight_format"):
                 continue
-            self._load(k, v)
+            self._load_target(k, v)
 
     def load_head_state_dict(self, sd: Dict[str, torch.Tensor], load_emb_from_target: bool = True):
         """Draft checkpoint keys as saved by the reference's trainers (strict=False like ea_model.py:76).
@@ -271,22 +288,24 @@ class EaModel(torch.nn.Module):
                         top_k=10, threshold=1.0, **kwargs):
         """Same signature as the reference (ea_model.py:88-170).  Reads an HF Llama checkpoint directory
         (config.json + safetensors / .bin shards) and a draft-head directory (config.json + pytorch_model.bin or
-        model.safetensors).  kwargs honoured: torch_dtype, max_length, device, tree_choices; HF placement knobs (`device_map`, `low_cpu_mem_usage`)
-        are accepted with a warning, anything else raises."""
-        from .checkpoint import iter_checkpoint_tensors, read_json
-        honoured = {"torch_dtype", "max_length", "device", "tree_choices"}
-        placement = {"device_map", "low_cpu_mem_usage", "load_in_8bit", "load_in_4bit"}  # HF / accelerate loading knobs
+        model.safetensors).  kwargs honoured: torch_dtype, max_length, device, tree_choices, load_in_8bit (int8 target projections,
+        eagle_b200.quant; a checkpoint saved in transformers' bitsandbytes 8-bit format loads its int8 values as stored);
+        HF placement knobs (`device_map`, `low_cpu_mem_usage`) are accepted with a warning, load_in_4bit and anything else raise."""
+        from .checkpoint import iter_checkpoint_tensors, iter_int8_pairs, read_json, target_weights_int8
+        honoured = {"torch_dtype", "max_length", "device", "tree_choices", "load_in_8bit", "load_in_4bit"}
+        placement = {"device_map", "low_cpu_mem_usage"}  # HF / accelerate loading knobs
         unknown = set(kwargs) - honoured - placement
         if unknown:
             raise TypeError(f"EaModel.from_pretrained: unsupported arguments {sorted(unknown)}")
         ignored = sorted(k for k in kwargs if k in placement and kwargs[k] not in (None, False))
-        if any(kwargs.get(k) for k in ("load_in_8bit", "load_in_4bit")):
-            raise ValueError("eagle_b200 runs bf16 / fp16 weights; quantised loading is not supported")
+        if kwargs.get("load_in_4bit"):
+            target_weights_int8({}, load_in_4bit=True)  # raises, naming what is supported
         if ignored:
             warnings.warn(f"eagle_b200 places the whole model on one GPU (`device`); ignoring {ignored}", stacklevel=2)
         tc = read_json(os.path.join(base_model_path, "config.json"))
         if tc.get("architectures", ["LlamaForCausalLM"])[0] != "LlamaForCausalLM":
             raise ValueError("eagle_b200 supports Llama-family targets (the configs named in BASELINE.json)")
+        int8 = target_weights_int8(tc, kwargs.get("load_in_8bit", False))
         hc = read_json(os.path.join(ea_model_path, "config.json"))
         dtype = kwargs.get("torch_dtype", torch.float16)
         tok = None
@@ -297,10 +316,15 @@ class EaModel(torch.nn.Module):
             tok = None
         m = cls(tc, hc, use_eagle3=use_eagle3, total_token=total_token, depth=depth, top_k=top_k, threshold=threshold,
                 torch_dtype=dtype, device=kwargs.get("device", 0), max_length=kwargs.get("max_length", 2048), tokenizer=tok,
-                tree_choices=kwargs.get("tree_choices"))
-        for k, v in iter_checkpoint_tensors(base_model_path):
-            if "rotary_emb" not in k:
+                tree_choices=kwargs.get("tree_choices"), load_in_8bit=int8)
+        for k, v, scb in iter_int8_pairs(base_model_path):
+            if "rotary_emb" in k:
+                continue
+            if scb is not None:  # stored bitsandbytes int8: loaded as is, not requantized
                 m._load(k, v)
+                m._load(k[: -len("weight")] + "SCB", scb)
+            else:
+                m._load_target(k, v)
         head_sd = dict(iter_checkpoint_tensors(ea_model_path, prefer_bin=True))
         m.load_head_state_dict(head_sd, load_emb_from_target=False)  # a checkpoint embed_tokens wins (ea_model.py:76)
         return m.finalize()

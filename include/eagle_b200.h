@@ -25,10 +25,10 @@
 extern "C" {
 #endif
 
-#define EB200_ABI_VERSION 1
+#define EB200_ABI_VERSION 2
 
 enum { EB200_BF16 = 0, EB200_FP16 = 1 };
-enum { EB200_DT_BF16 = 0, EB200_DT_FP16 = 1, EB200_DT_FP32 = 2, EB200_DT_INT64 = 3, EB200_DT_BOOL = 4 };
+enum { EB200_DT_BF16 = 0, EB200_DT_FP16 = 1, EB200_DT_FP32 = 2, EB200_DT_INT64 = 3, EB200_DT_BOOL = 4, EB200_DT_INT8 = 5 };
 
 typedef struct eb200_engine eb200_engine;
 
@@ -61,6 +61,12 @@ typedef struct eb200_config {
 #define EB200_FLAG_SIMT_GEMM 1   /* bring-up only: route GEMMs through the plain-FMA kernel */
 #define EB200_FLAG_NO_GRAPH 2    /* launch kernels directly instead of replaying the captured cycle graph */
 #define EB200_FLAG_NO_CHAIN 4    /* one kernel per projection / RMSNorm instead of the persistent per-layer chain launches */
+/* The q/k/v/o/gate/up/down projections of every TARGET decoder layer are stored as int8 plus one fp32 scale per row
+ * (bitsandbytes' 8-bit weight format) and multiplied by a W8A16 GEMM that computes exactly what the model-dtype GEMM computes on
+ * W' = dtype((q * SCB) * 7.874015718698502e-3).  lm_head, embeddings, norms and the draft head stay in the model dtype.
+ * Single GPU, default GEMM path only: eb200_finalize refuses tp_size > 1, EB200_FLAG_SIMT_GEMM, EB200_CHAIN=1 and
+ * EB200_GEMM_MODE=streamk. */
+#define EB200_FLAG_TARGET_INT8 8
 
 typedef struct eb200_gen_params {
   float temperature, top_p;   /* eagenerate(temperature, top_p, top_k, ...) ea_model.py:199-208 */
@@ -87,7 +93,10 @@ void eb200_destroy(eb200_engine* e);
  *            "head.fc.weight", "head.midlayer.self_attn.q_proj.weight", "head.lm_head.weight", "head.d2t",
  *            "head.embed_tokens.weight" (optional: defaults to the target embedding, ea_model.py:55-60 load_emb)
  * `data` is the FULL tensor (host or device, row-major, `dtype` as given); with tp_size > 1 the engine keeps only
- * this rank's shard.  shape has ndim entries. */
+ * this rank's shard.  shape has ndim entries.
+ * EB200_FLAG_TARGET_INT8 engines take each target projection as "model.layers.{i}.<proj>.weight" in EB200_DT_INT8 [out, in]
+ * plus "model.layers.{i}.<proj>.SCB" in EB200_DT_FP32 [out] (its row absmax, the key transformers serializes bnb 8-bit models
+ * with); model-dtype data for those names is rejected, and so is int8 data anywhere else or for an engine without the flag. */
 int eb200_load_tensor(eb200_engine* e, const char* name, const void* data, const int64_t* shape, int32_t ndim,
                       int32_t dtype);
 /* cos/sin tables [n_pos][head_dim/2] in the model dtype, built by the caller exactly like the reference's
@@ -192,6 +201,10 @@ int eb200_reset_stats(eb200_engine* e);
  * All pointers are DEVICE pointers unless noted; dtype is EB200_BF16/FP16. */
 int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const void* W, const void* W2, const void* X, void* out,
                  const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
+/* the W8A16 cluster split-K GEMM (EB200_FLAG_TARGET_INT8): Wq int8 [N, K], scb fp32 [N]; epilogue codes and M <= 64 as
+ * eb200_k_gemm (0 store, 1 residual, 5 interleaved SwiGLU with N output columns over a [2N, K] weight); bias: store only */
+int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, const void* scb, const void* X, void* out, const void* res,
+                    const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
 /* micro-benchmark of the skinny GEMM: `iters` back-to-back launches cycling over `n_weights` distinct [N,K] weight
  * matrices (so the stream is HBM-, not L2-resident), timed with CUDA events; optionally replayed from a CUDA graph.
  * epilogue: 0 store, 1 residual, 2 swiglu.  Returns the average microseconds per launch. */
