@@ -103,7 +103,8 @@ __device__ __forceinline__ int sw_off(int r, int c) {
 
 template <typename T, int HPC>
 __global__ void __launch_bounds__(kThreads) tree_attention_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                                                                  const AttnParams p, int kv_stride, int kvs) {
+                                                                  const AttnParams p, int kv_stride, int kvs,
+                                                                  const __grid_constant__ L2Prefetch pf) {
   using D = DT<T>;
   constexpr int CS = kWarps / HPC;         // warps sharing one query head (column / output-dim split)
   constexpr int NT1 = (kKvTile / CS) / 8;  // n8 score tiles per warp per kv tile
@@ -119,22 +120,9 @@ __global__ void __launch_bounds__(kThreads) tree_attention_kernel(const __grid_c
   float* sPO = reinterpret_cast<float*>(sRing);         // [HPC*16][128] partial outputs (aliases the ring after the sweeps)
 
   pdl_launch_dependents();
-  if (threadIdx.x == 0) {
-    // weights are immutable: prefetching them needs no dependency wait
-    const unsigned long long n_cta = static_cast<unsigned long long>(gridDim.x) * gridDim.y * gridDim.z;
-    const unsigned long long cta = blockIdx.x + static_cast<unsigned long long>(gridDim.x) * (blockIdx.y + static_cast<unsigned long long>(gridDim.y) * blockIdx.z);
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      if (!p.pf_ptr[r] || !p.pf_bytes[r]) continue;
-      const unsigned long long per = ((p.pf_bytes[r] + n_cta - 1) / n_cta + 4095ull) & ~4095ull;
-      unsigned long long off = cta * per;
-      const unsigned long long end = min(p.pf_bytes[r], off + per);
-      for (; off < end; off += 16384ull) {
-        const unsigned int sz = static_cast<unsigned int>(min(16384ull, end - off)) & ~15u;
-        if (sz)
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<const char*>(p.pf_ptr[r]) + off), "r"(sz) : "memory");
-      }
-    }
+  if (threadIdx.x < 32) {  // weights are immutable: prefetching them needs no dependency wait
+    const int cta = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
+    l2_prefetch_weights(pf, cta * 32 + threadIdx.x, gridDim.x * gridDim.y * gridDim.z * 32);
   }
   unsigned long long* tr = nullptr;
   unsigned long long t_launch = 0;
@@ -519,7 +507,9 @@ template <typename T, int HPC> static int launch_hpc(const AttnParams& p, int kv
     configured_dev[cur_dev] = true;
   }
   dim3 grid(p.n_heads / HPC, (p.rows + 15) / 16, kvs);
-  return static_cast<int>(launch_kc(kern, grid, dim3(kThreads), smem, s, dim3(1, 1, kvs), *p.tmK, *p.tmV, p, kv_stride, kvs));
+  L2Prefetch none;
+  memset(&none, 0, sizeof(none));
+  return static_cast<int>(launch_kc(kern, grid, dim3(kThreads), smem, s, dim3(1, 1, kvs), *p.tmK, *p.tmV, p, kv_stride, kvs, p.pf ? *p.pf : none));
 }
 
 int launch_attention(int dtype, const AttnParams& p, cudaStream_t s) {

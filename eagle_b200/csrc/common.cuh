@@ -14,6 +14,8 @@
 
 #include <utility>
 
+#include "kernels.h"
+
 #if defined(__CUDA_ARCH__) && !defined(__CUDA_ARCH_FEAT_SM90_ALL)
 #error "eagle_b200 kernels are written for sm_90a (wgmma / TMA / clusters)"
 #endif
@@ -113,6 +115,27 @@ constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
 
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
+}
+// global -> L2 only, the same box a tma_load_2d of (c0, c1) would load; boxes past the tensor's bounds are clipped by the map
+__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1)
+               : "memory");
+}
+// Worker w of n issues boxes w, w + n, ... of an L2Prefetch plan (kernels.h), in the consuming GEMM's order.  pf must be a
+// __grid_constant__ kernel parameter (the map is read from the parameter bank).  No dependency on earlier kernels, so it may
+// precede griddepcontrol.wait.  The lines keep the default L2 policy; the GEMM's own evict-first loads do not demote them.
+__device__ __forceinline__ void l2_prefetch_weights(const L2Prefetch& pf, int worker, int n_workers) {
+  const int per_j = pf.n_tiles * pf.splitk;
+  const int j0 = max(pf.j0, 0);
+  if (per_j <= 0 || pf.j1 <= j0) return;
+  const int total = (pf.j1 - j0) * per_j;
+  for (int u = worker; u < total; u += n_workers) {
+    const int j = j0 + u / per_j, r = u % per_j;
+    const int split = r / pf.n_tiles, tile = r - split * pf.n_tiles;
+    const int kb = static_cast<int>((static_cast<long>(pf.num_kb) * split) / pf.splitk) + j;
+    const int kb_end = static_cast<int>((static_cast<long>(pf.num_kb) * (split + 1)) / pf.splitk);
+    if (kb < kb_end) tma_prefetch_l2_2d(&pf.tm, kb * 64, tile * 128);
+  }
 }
 // 2-D tile load global -> shared, completion signalled on an mbarrier (complete_tx::bytes)
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,

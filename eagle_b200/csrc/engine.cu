@@ -190,6 +190,7 @@ struct eb200_engine {
   // split-K
   float* ws = nullptr;
   size_t ws_bytes = 0;
+  size_t l2_bytes = 0;  // device L2 size: caps the weight bytes prefetched ahead of a GEMM
   float* sk_ws = nullptr;  // stream-K partial slots
   int* counters = nullptr;
   // tree + cycle state
@@ -332,6 +333,7 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
   eb200_engine* e = new eb200_engine();
   e->c = c;
   e->dtype = c.dtype;
+  e->l2_bytes = static_cast<size_t>(prop.l2CacheSize);
   memset(&e->stats, 0, sizeof(e->stats));
   {
     cudaError_t se = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
@@ -1041,12 +1043,53 @@ static int gemm_mode() {
   return v;
 }
 
+// EB200_L2_PREFETCH=1 turns the L2 weight prefetch on; read once.  Off by default: on the H100 every window measured slower with
+// it (DESIGN.md §5), so it stays an experiment.
+static bool l2_prefetch_on() {
+  static int v = -1;
+  if (v < 0) {
+    const char* s = getenv("EB200_L2_PREFETCH");
+    v = (s && atoi(s) == 1) ? 1 : 0;
+  }
+  return v == 1;
+}
+// Bytes a GEMM's drain and an RMSNorm / e3_input window prefetch of the GEMM that follows (about their idle time x HBM rate), and
+// the cap on what is prefetched ahead of one GEMM in all, as a share of L2 (the live working set besides is a few MB).
+static double pf_tail_bytes() { return 8.0 * (1 << 20); }
+static double pf_norm_bytes() { return 8.0 * (1 << 20); }
+static double pf_cap_share() { return 0.5; }
+// Plan (kernels.h L2Prefetch) over the weight of `next`, the GEMM launched next over it at `mpad` rows: its k-block rows
+// [j0, j0 + about `bytes`), with the same grid (pick_splitk) as that launch.  The plan ends at the matrix, and at the L2 cap
+// counted from row 0; pf.j1 is where a later window's plan over the same GEMM continues.
+static int pick_splitk(int N, int K, int mpad, int epi, size_t ws_bytes);
+static L2Prefetch l2_plan(const eb200_engine* e, const Linear& next, int mpad, int j0, double bytes) {
+  L2Prefetch pf;
+  memset(&pf, 0, sizeof(pf));
+  pf.j0 = pf.j1 = j0;
+  if (!l2_prefetch_on() || !next.w || next.N <= 0 || next.K <= 0 || bytes <= 0) return pf;
+  pf.tm = next.tm;
+  pf.n_tiles = (next.N + 127) / 128;
+  pf.splitk = pick_splitk(next.N, next.K, mpad, 0, e->ws_bytes);
+  pf.num_kb = (next.K + 63) / 64;
+  const double row = static_cast<double>(pf.n_tiles) * pf.splitk * 128 * 64 * next.esize;  // one k-block of every (n-tile, split)
+  const int rows_all = (pf.num_kb + pf.splitk - 1) / pf.splitk;
+  const int rows_cap = static_cast<int>(static_cast<double>(e->l2_bytes) * pf_cap_share() / row);
+  const int rows = std::max(1, static_cast<int>(bytes / row));
+  pf.j1 = std::max(j0, std::min({rows_all, rows_cap, j0 + rows}));
+  return pf;
+}
+// the rest of the L2 cap over the same GEMM, after `prev`
+static L2Prefetch l2_plan_rest(const eb200_engine* e, const Linear& next, int mpad, const L2Prefetch& prev) {
+  return l2_plan(e, next, mpad, prev.j1, static_cast<double>(e->l2_bytes));
+}
+
 struct GemmCall {
   const Linear* W;
   const Linear* W2;
   const ActBuf* X;
   int epi;
   GemmParams p;
+  const L2Prefetch* pf;  // optional: the next GEMM's leading weight tiles, prefetched by this launch's producers after their last load
 };
 static bool skip_kernel(const char* name);
 static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
@@ -1074,7 +1117,7 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
   if (p.w_scale) {
     if (cx.mpad == 256 && g.X->rows < 256) return fail("256-row GEMM on a 64-row activation buffer");
     CKL(launch_gemm_w8(e->dtype, cx.mpad, g.epi, &g.W->tm, cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256), p,
-                       e->stream));
+                       e->stream, g.pf));
   } else if (e->c.flags & EB200_FLAG_SIMT_GEMM) {
     const size_t per_split = static_cast<size_t>(g.epi == EPI_SWIGLU ? 2 : 1) * cx.mpad * ((p.N + 127) / 128) * 128 * 4;
     while (p.splitk > 1 && per_split * p.splitk > e->ws_bytes) --p.splitk;
@@ -1082,23 +1125,26 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
   } else if (gemm_mode() == 1) {
     if (cx.mpad == 256 && g.X->rows < 256) return fail("256-row GEMM on a 64-row activation buffer");
     CKL(launch_gemm(e->dtype, cx.mpad, g.epi, &g.W->tm, g.W2 ? &g.W2->tm : nullptr,
-                    cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256), p, e->stream, cx.mpad == 64 ? &g.X->tm32 : nullptr));
+                    cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256), p, e->stream, cx.mpad == 64 ? &g.X->tm32 : nullptr,
+                    g.pf));
   } else {
     CKL(launch_gemm_streamk(e->dtype, cx.mpad, g.epi, &g.W->tm, g.W2 ? &g.W2->tm : nullptr, cx.mpad == 16 ? &g.X->tm16 : &g.X->tm64, p,
                             e->sk_ws, e->counters, e->stream));
   }
   return 0;
 }
-static int gemm_store(eb200_engine* e, const RowCtx& cx, const Linear& W, const ActBuf& X, void* out, long ld, const void* bias) {
-  GemmCall g{&W, nullptr, &X, EPI_STORE, {}};
+static int gemm_store(eb200_engine* e, const RowCtx& cx, const Linear& W, const ActBuf& X, void* out, long ld, const void* bias,
+                      const L2Prefetch* pf = nullptr) {
+  GemmCall g{&W, nullptr, &X, EPI_STORE, {}, pf};
   memset(&g.p, 0, sizeof(g.p));
   g.p.out = out;
   g.p.ld_out = ld;
   g.p.bias = bias;
   return run_gemm(e, cx, g);
 }
-static int gemm_residual(eb200_engine* e, const RowCtx& cx, const Linear& W, const ActBuf& X, const void* res, void* out, long ld) {
-  GemmCall g{&W, nullptr, &X, EPI_RESIDUAL, {}};
+static int gemm_residual(eb200_engine* e, const RowCtx& cx, const Linear& W, const ActBuf& X, const void* res, void* out, long ld,
+                         const L2Prefetch* pf = nullptr) {
+  GemmCall g{&W, nullptr, &X, EPI_RESIDUAL, {}, pf};
   memset(&g.p, 0, sizeof(g.p));
   g.p.out = out;
   g.p.ld_out = ld;
@@ -1106,16 +1152,17 @@ static int gemm_residual(eb200_engine* e, const RowCtx& cx, const Linear& W, con
   g.p.ld_res = ld;
   return run_gemm(e, cx, g);
 }
-static int gemm_swiglu(eb200_engine* e, const RowCtx& cx, const Linear& Wgu, const ActBuf& X, void* out, long ld) {
-  GemmCall g{&Wgu, nullptr, &X, EPI_SWIGLU_IL, {}};
+static int gemm_swiglu(eb200_engine* e, const RowCtx& cx, const Linear& Wgu, const ActBuf& X, void* out, long ld,
+                       const L2Prefetch* pf = nullptr) {
+  GemmCall g{&Wgu, nullptr, &X, EPI_SWIGLU_IL, {}, pf};
   memset(&g.p, 0, sizeof(g.p));
   g.p.out = out;
   g.p.ld_out = ld;
   return run_gemm(e, cx, g);
 }
 static int gemm_qkv(eb200_engine* e, const RowCtx& cx, const Linear& W, const ActBuf& X, void* q_out, void* kc, void* vc, long cap,
-                    int nq, int nkv, const void* cosp, const void* sinp) {
-  GemmCall g{&W, nullptr, &X, EPI_QKV_ROPE, {}};
+                    int nq, int nkv, const void* cosp, const void* sinp, const L2Prefetch* pf = nullptr) {
+  GemmCall g{&W, nullptr, &X, EPI_QKV_ROPE, {}, pf};
   memset(&g.p, 0, sizeof(g.p));
   g.p.q_out = q_out;
   g.p.k_cache = kc;
@@ -1131,8 +1178,9 @@ static int gemm_qkv(eb200_engine* e, const RowCtx& cx, const Linear& W, const Ac
   g.p.kv_base = cx.kv_base;
   return run_gemm(e, cx, g);
 }
-static int gemm_partial_f32(eb200_engine* e, const RowCtx& cx, const Linear& W, const ActBuf& X, float* out, long ld) {
-  GemmCall g{&W, nullptr, &X, EPI_PARTIAL_F32, {}};
+static int gemm_partial_f32(eb200_engine* e, const RowCtx& cx, const Linear& W, const ActBuf& X, float* out, long ld,
+                            const L2Prefetch* pf = nullptr) {
+  GemmCall g{&W, nullptr, &X, EPI_PARTIAL_F32, {}, pf};
   memset(&g.p, 0, sizeof(g.p));
   g.p.out = out;
   g.p.ld_out = ld;
@@ -1148,10 +1196,10 @@ static void chain_fill_tp(eb200_engine* e, ChainArgs& a);
 //     every rank (tp_fused.cu) -- *did_norm tells the caller that xn is already there; or
 //   * NCCL: all-reduce, then the residual add; the caller runs the RMSNorm.
 static int row_parallel_residual(eb200_engine* e, const RowCtx& cx, const Linear& W, const ActBuf& X, void* x, int H, const void* norm_w = nullptr,
-                                 void* tap = nullptr, bool* did_norm = nullptr) {
+                                 void* tap = nullptr, bool* did_norm = nullptr, const L2Prefetch* pf = nullptr) {
   if (did_norm) *did_norm = false;
-  if (e->c.tp_size == 1) return gemm_residual(e, cx, W, X, x, x, H);
-  TRY(gemm_partial_f32(e, cx, W, X, e->f32buf, H));
+  if (e->c.tp_size == 1) return gemm_residual(e, cx, W, X, x, x, H, pf);
+  TRY(gemm_partial_f32(e, cx, W, X, e->f32buf, H, pf));
   if (e->tp_fused && cx.rows_idx < 0) {
     TpResidParams p;
     memset(&p, 0, sizeof(p));
@@ -1273,10 +1321,10 @@ static bool skip_kernel(const char* name) {
 }
 
 static int rmsnorm(eb200_engine* e, const void* src, long ld_src, const int64_t* ids64, const int* ids32, const void* w, void* y,
-                   long ld_y, int col_off, int H, float eps, int rows) {
+                   long ld_y, int col_off, int H, float eps, int rows, const L2Prefetch* pf = nullptr) {
   if (skip_kernel("rmsnorm")) return 0;
   ProfScope ps(e, 2, 0, "rmsnorm");
-  CKL(launch_rmsnorm(e->dtype, src, ld_src, ids64, ids32, w, y, ld_y, col_off, H, eps, rows, e->stream));
+  CKL(launch_rmsnorm(e->dtype, src, ld_src, ids64, ids32, w, y, ld_y, col_off, H, eps, rows, e->stream, pf));
   return 0;
 }
 static int gather(eb200_engine* e, const void* table, long ld_table, const int64_t* ids64, const int* ids32, void* dst, long ld_dst,
@@ -1286,7 +1334,7 @@ static int gather(eb200_engine* e, const void* table, long ld_table, const int64
   return 0;
 }
 static int attention(eb200_engine* e, const RowCtx& cx, const void* q, void* kc, void* vc, void* out, long cap, int nh, int nkv,
-                     const Linear* next0 = nullptr, const Linear* next1 = nullptr) {
+                     const L2Prefetch* pf = nullptr) {
   if (skip_kernel("attention")) return 0;
   if (cx.rows > 64) {
     // a causal prompt chunk of up to 256 rows: the kernel's ancestor mask covers 128 new columns, so the chunk is attended in
@@ -1300,29 +1348,13 @@ static int attention(eb200_engine* e, const RowCtx& cx, const void* q, void* kc,
       sub.n_tree = sub.rows;
       sub.kv_bound = cx.kv_bound > 0 ? std::min(cx.kv_bound, cx.kv_bound - cx.rows + r0 + sub.rows) : 0;
       const size_t off = static_cast<size_t>(r0) * nh * 128 * 2;
-      TRY(attention(e, sub, reinterpret_cast<const char*>(q) + off, kc, vc, reinterpret_cast<char*>(out) + off, cap, nh, nkv, nullptr, nullptr));
+      TRY(attention(e, sub, reinterpret_cast<const char*>(q) + off, kc, vc, reinterpret_cast<char*>(out) + off, cap, nh, nkv, r0 == 0 ? pf : nullptr));
     }
     return 0;
   }
   AttnParams a;
   memset(&a, 0, sizeof(a));
-  {
-    // L2 prefetch budget for the weights the following chain launch streams first (EB200_ATTN_PREFETCH_MB, 0 = off)
-    static long budget = -1;
-    if (budget < 0) {
-      const char* s = getenv("EB200_ATTN_PREFETCH_MB");
-      budget = (s ? atol(s) : 0) << 20;  // off by default (an experiment knob)
-    }
-    long left = budget;
-    const Linear* nx[2] = {next0, next1};
-    for (int r = 0; r < 2; ++r) {
-      if (!nx[r] || left <= 0) continue;
-      const long bytes = std::min<long>(left, static_cast<long>(nx[r]->N) * nx[r]->K * nx[r]->esize);
-      a.pf_ptr[r] = nx[r]->w;
-      a.pf_bytes[r] = static_cast<unsigned long long>(bytes);
-      left -= bytes;
-    }
-  }
+  a.pf = pf;
   a.trace = e->in_verify ? e->attn_trace : nullptr;
   a.q = q;
   a.k_cache = kc;
@@ -1673,7 +1705,8 @@ static int target_forward(eb200_engine* e, const RowCtx& cx, const int64_t* ids6
     for (int i = 0; i < L; ++i) {
       void* kc = kv_plane(e->t_kv, i, 0, e->nkv_l, e->cap);
       void* vc = kv_plane(e->t_kv, i, 1, e->nkv_l, e->cap);
-      TRY(attention(e, cx, e->q, kc, vc, e->attn.p, e->cap, e->nh_l, e->nkv_l, &e->tl[i].o, &e->tl[i].gu));
+      const L2Prefetch pf_o = l2_plan(e, e->tl[i].o, cx.mpad, 0, static_cast<double>(e->l2_bytes));  // the chain's first phase
+      TRY(attention(e, cx, e->q, kc, vc, e->attn.p, e->cap, e->nh_l, e->nkv_l, &pf_o));
       TRY(target_segment_chain(e, cx, i, feat_dst, &slot, head_mode));
     }
     if (!e->c.eagle3 && feat_dst) TRY(gather(e, e->xn.p, H, nullptr, e->ident, feat_dst, e->F, 0, H, cx.rows));
@@ -1682,25 +1715,40 @@ static int target_forward(eb200_engine* e, const RowCtx& cx, const int64_t* ids6
   }
   bool have_xn = false;   // xn already holds this layer's input_layernorm(x) (written by the previous down_proj's fused TP kernel)
   bool tap_done = false;  // ... and the EAGLE-3 tap of this layer was written there too
+  // L2 prefetch: every GEMM's producers fetch the leading weight tiles of the next GEMM after their last load, and the latency-bound
+  // kernel in between (RMSNorm, attention) continues where that plan ends
+  L2Prefetch pf_qkv_head;  // the part of this layer's qkv the previous down_proj prefetched
+  memset(&pf_qkv_head, 0, sizeof(pf_qkv_head));
   for (int i = 0; i < L; ++i) {
     Layer& l = e->tl[i];
     if (e->c.eagle3 && feat_dst && is_tap_layer(e, i)) {
       if (!tap_done) TRY(gather(e, e->x, H, nullptr, e->ident, feat_dst, e->F, slot * H, H, cx.rows));
       ++slot;
     }
-    if (!have_xn) TRY(rmsnorm(e, e->x, H, nullptr, nullptr, l.ln1, e->xn.p, H, 0, H, eps, cx.rows));
+    if (!have_xn) {
+      const L2Prefetch pf = l2_plan(e, l.qkv, cx.mpad, pf_qkv_head.j1, pf_norm_bytes());
+      TRY(rmsnorm(e, e->x, H, nullptr, nullptr, l.ln1, e->xn.p, H, 0, H, eps, cx.rows, &pf));
+    }
     void* kc = kv_plane(e->t_kv, i, 0, e->nkv_l, e->cap);
     void* vc = kv_plane(e->t_kv, i, 1, e->nkv_l, e->cap);
-    TRY(gemm_qkv(e, cx, l.qkv, e->xn, e->q, kc, vc, e->cap, e->nh_l, e->nkv_l, e->t_cos, e->t_sin));
-    TRY(attention(e, cx, e->q, kc, vc, e->attn.p, e->cap, e->nh_l, e->nkv_l));
+    const L2Prefetch pf_o = l2_plan(e, l.o, cx.mpad, 0, pf_tail_bytes());
+    TRY(gemm_qkv(e, cx, l.qkv, e->xn, e->q, kc, vc, e->cap, e->nh_l, e->nkv_l, e->t_cos, e->t_sin, &pf_o));
+    const L2Prefetch pf_o_rest = l2_plan_rest(e, l.o, cx.mpad, pf_o);
+    TRY(attention(e, cx, e->q, kc, vc, e->attn.p, e->cap, e->nh_l, e->nkv_l, &pf_o_rest));
     bool did = false;
-    TRY(row_parallel_residual(e, cx, l.o, e->attn, e->x, H, l.ln2, nullptr, &did));
-    if (!did) TRY(rmsnorm(e, e->x, H, nullptr, nullptr, l.ln2, e->xn.p, H, 0, H, eps, cx.rows));
-    TRY(gemm_swiglu(e, cx, l.gu, e->xn, e->act.p, e->I_l));
+    const L2Prefetch pf_gu = l2_plan(e, l.gu, cx.mpad, 0, pf_tail_bytes());
+    TRY(row_parallel_residual(e, cx, l.o, e->attn, e->x, H, l.ln2, nullptr, &did, &pf_gu));
+    if (!did) {
+      const L2Prefetch pf = l2_plan(e, l.gu, cx.mpad, pf_gu.j1, pf_norm_bytes());
+      TRY(rmsnorm(e, e->x, H, nullptr, nullptr, l.ln2, e->xn.p, H, 0, H, eps, cx.rows, &pf));
+    }
+    const L2Prefetch pf_down = l2_plan(e, l.down, cx.mpad, 0, pf_tail_bytes());
+    TRY(gemm_swiglu(e, cx, l.gu, e->xn, e->act.p, e->I_l, &pf_down));
     const void* next_norm = (i + 1 < L) ? e->tl[i + 1].ln1 : e->t_norm;
     void* tap = nullptr;
     if (e->c.eagle3 && feat_dst && i + 1 < L && is_tap_layer(e, i + 1)) tap = reinterpret_cast<char*>(feat_dst) + static_cast<size_t>(slot) * H * 2;
-    TRY(row_parallel_residual(e, cx, l.down, e->act, e->x, H, next_norm, tap, &did));
+    pf_qkv_head = i + 1 < L ? l2_plan(e, e->tl[i + 1].qkv, cx.mpad, 0, pf_tail_bytes()) : l2_plan(e, l.qkv, cx.mpad, 0, 0);
+    TRY(row_parallel_residual(e, cx, l.down, e->act, e->x, H, next_norm, tap, &did, &pf_qkv_head));
     have_xn = did;
     tap_done = did && tap != nullptr;
   }
@@ -1790,12 +1838,15 @@ static int draft_forward(eb200_engine* e, const RowCtx& cx, const int64_t* ids64
   const float eps = e->c.head_rms_norm_eps;
   if (e->c.eagle3) {
     Layer& l = e->hl[0];
-    if (first_pass) TRY(gemm_store(e, cx, e->h_fc, e->d_feat, e->d_h.p, Hh, nullptr));  // cnets.py:639-640
+    // L2 prefetch as in target_forward.  The qkv's head is prefetched by the fc (first pass) or by the previous pass' lm_head.
+    const L2Prefetch pf_qkv_head = l2_plan(e, l.qkv, cx.mpad, 0, pf_tail_bytes());
+    if (first_pass) TRY(gemm_store(e, cx, e->h_fc, e->d_feat, e->d_h.p, Hh, nullptr, &pf_qkv_head));  // cnets.py:639-640
     // cat(norm(emb(ids)), norm(hidden))  cnets.py:427-430
     if (e->fused_e3_input) {
       ProfScope ps(e, 2, 0, "e3_input");
+      const L2Prefetch pf = l2_plan(e, l.qkv, cx.mpad, pf_qkv_head.j1, pf_norm_bytes());
       CKL(launch_e3_input(e->dtype, e->h_embed, Hh, ids64, ids32, l.ln1, src_rows ? e->d_out.p : e->d_h.p, Hh, src_rows, e->d_h.p, Hh,
-                          e->h_hidden_norm, e->d_cat.p, 2 * Hh, Hh, eps, cx.rows, e->stream));
+                          e->h_hidden_norm, e->d_cat.p, 2 * Hh, Hh, eps, cx.rows, e->stream, &pf));
     } else {
       if (src_rows) TRY(gather(e, e->d_out.p, Hh, nullptr, src_rows, e->d_h.p, Hh, 0, Hh, cx.rows));
       TRY(rmsnorm(e, e->h_embed, Hh, ids64, ids32, l.ln1, e->d_cat.p, 2 * Hh, 0, Hh, eps, cx.rows));
@@ -1803,16 +1854,24 @@ static int draft_forward(eb200_engine* e, const RowCtx& cx, const int64_t* ids64
     }
     void* kc = kv_plane(e->d_kv, 0, 0, e->hnkv, e->dcap);
     void* vc = kv_plane(e->d_kv, 0, 1, e->hnkv, e->dcap);
-    TRY(gemm_qkv(e, cx, l.qkv, e->d_cat, e->d_q, kc, vc, e->dcap, e->hnh, e->hnkv, e->h_cos, e->h_sin));
-    TRY(attention(e, cx, e->d_q, kc, vc, e->d_attn.p, e->dcap, e->hnh, e->hnkv, e->chain_draft ? &l.o : nullptr, e->chain_draft ? &l.gu : nullptr));
+    const L2Prefetch pf_o = l2_plan(e, l.o, cx.mpad, 0, e->chain_draft ? 0 : pf_tail_bytes());
+    TRY(gemm_qkv(e, cx, l.qkv, e->d_cat, e->d_q, kc, vc, e->dcap, e->hnh, e->hnkv, e->h_cos, e->h_sin, &pf_o));
+    const L2Prefetch pf_o_rest = l2_plan_rest(e, l.o, cx.mpad, pf_o);
+    TRY(attention(e, cx, e->d_q, kc, vc, e->d_attn.p, e->dcap, e->hnh, e->hnkv, &pf_o_rest));
     if (e->chain_draft) return draft_segment_chain(e, cx, 0);
-    TRY(gemm_residual(e, cx, l.o, e->d_attn, e->d_h.p, e->d_h2, Hh));
-    TRY(rmsnorm(e, e->d_h2, Hh, nullptr, nullptr, l.ln2, e->d_xn.p, Hh, 0, Hh, eps, cx.rows));
-    TRY(gemm_swiglu(e, cx, l.gu, e->d_xn, e->d_act.p, e->Ih));
-    TRY(gemm_residual(e, cx, l.down, e->d_act, e->d_h2, e->d_out.p, Hh));
+    const L2Prefetch pf_gu = l2_plan(e, l.gu, cx.mpad, 0, pf_tail_bytes());
+    TRY(gemm_residual(e, cx, l.o, e->d_attn, e->d_h.p, e->d_h2, Hh, &pf_gu));
+    const L2Prefetch pf_gu_rest = l2_plan(e, l.gu, cx.mpad, pf_gu.j1, pf_norm_bytes());
+    TRY(rmsnorm(e, e->d_h2, Hh, nullptr, nullptr, l.ln2, e->d_xn.p, Hh, 0, Hh, eps, cx.rows, &pf_gu_rest));
+    const L2Prefetch pf_down = l2_plan(e, l.down, cx.mpad, 0, pf_tail_bytes());
+    TRY(gemm_swiglu(e, cx, l.gu, e->d_xn, e->d_act.p, e->Ih, &pf_down));
+    const L2Prefetch pf_head = l2_plan(e, e->h_head, cx.mpad, 0, pf_tail_bytes());
+    TRY(gemm_residual(e, cx, l.down, e->d_act, e->d_h2, e->d_out.p, Hh, &pf_head));
     // lm_head(norm(out))  cnets.py:700, :734
-    TRY(rmsnorm(e, e->d_out.p, Hh, nullptr, nullptr, e->h_norm, e->d_xn.p, Hh, 0, Hh, eps, cx.rows));
-    TRY(gemm_store(e, cx, e->h_head, e->d_xn, e->d_logits, e->Vd, nullptr));
+    const L2Prefetch pf_head_rest = l2_plan(e, e->h_head, cx.mpad, pf_head.j1, pf_norm_bytes());
+    TRY(rmsnorm(e, e->d_out.p, Hh, nullptr, nullptr, e->h_norm, e->d_xn.p, Hh, 0, Hh, eps, cx.rows, &pf_head_rest));
+    // the next draft pass starts with the same qkv (after the level's top-k / tree kernels and e3_input)
+    TRY(gemm_store(e, cx, e->h_head, e->d_xn, e->d_logits, e->Vd, nullptr, &pf_qkv_head));
     return 0;
   }
   // EAGLE-1/2: fc(cat(emb, hidden)) (cnets1.py:623), layer 0 without input norm (:428-429), target lm_head (:702,:732)
@@ -2657,6 +2716,45 @@ extern "C" int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const
       if (!skws) return fail("scratch allocation failed");
       CKL(launch_gemm_streamk(dtype, mpad, epilogue, &tw, W2 ? &tw2 : nullptr, &tx, p, skws, counters, s));
     }
+  }
+  CK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+extern "C" int eb200_k_prefetch(int32_t dtype, int32_t kernel, int32_t epilogue, const void* W, const void* X, void* out, const void* res,
+                                int32_t M, int32_t N, int32_t K, int32_t splitk, float eps, const void* P, int32_t PN, int32_t PK,
+                                int32_t p_splitk, int32_t j0, int32_t j1, void* stream) {
+  if (M < 1 || M > 64 || N < 1 || !P || PN < 1 || PK < 1 || p_splitk < 1 || p_splitk > 8 || kernel < 0 || kernel > 1 ||
+      (kernel == 0 && (K < 1 || splitk < 1 || splitk > 8 || (epilogue != EPI_STORE && epilogue != EPI_RESIDUAL))))
+    return fail("eb200_k_prefetch: bad arguments");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  L2Prefetch pf;
+  memset(&pf, 0, sizeof(pf));
+  TRY(make_tmap(&pf.tm, dtype, P, PN, PK, 128));
+  pf.n_tiles = (PN + 127) / 128;
+  pf.splitk = p_splitk;
+  pf.num_kb = (PK + 63) / 64;
+  pf.j0 = j0;
+  pf.j1 = j1;
+  if (kernel == 1) {
+    CKL(launch_rmsnorm(dtype, X, N, nullptr, nullptr, W, out, N, 0, N, eps, M, s, &pf));
+  } else {
+    const int mpad = M <= 16 ? 16 : 64;
+    GemmParams p;
+    memset(&p, 0, sizeof(p));
+    p.N = N;
+    p.K = K;
+    p.m_rows = M;
+    p.m_idx = -1;
+    p.splitk = splitk;
+    p.out = out;
+    p.ld_out = N;
+    p.res = res;
+    p.ld_res = N;
+    CUtensorMap tw, tx;
+    TRY(make_tmap(&tw, dtype, W, N, K, 128));
+    TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
+    CKL(launch_gemm(dtype, mpad, epilogue, &tw, nullptr, &tx, p, s, nullptr, &pf));
   }
   CK(cudaStreamSynchronize(s));
   return 0;

@@ -26,8 +26,10 @@
 
 namespace eb {
 
-// Stage memory per CTA.  Grids that fit one CTA per SM get a deep ring (one resident CTA, ~200 KB in flight);
-// larger grids run two CTAs per SM with ~100 KB each so one CTA's prologue/epilogue hides under the other's loop.
+// Stage memory per CTA: ~100 KB, so two CTAs fit on an SM.  For grids larger than the SM count one CTA's prologue/epilogue hides
+// under the other's loop.  Grids that fit one CTA per SM (EB200_GEMM_SMEM_BIG_KB) take the same budget: the next kernel's CTAs then
+// become resident next to them and fill their own rings while these drain.  With a 200 KB ring they waited for these to exit, and
+// the cycle was 5 % slower on the H100 (DESIGN.md §5).
 static int env_kb(const char* name, int dflt) {
   const char* e = getenv(name);
   int kb = e ? atoi(e) : dflt;
@@ -39,7 +41,7 @@ static int smem_budget(int total_ctas) {
   static int small_kb = 0, big_kb = 0;
   if (!small_kb) {
     small_kb = env_kb("EB200_GEMM_SMEM_KB", 100);      // when the grid exceeds the SM count (two per SM)
-    big_kb = env_kb("EB200_GEMM_SMEM_BIG_KB", 200);    // when it fits one CTA per SM
+    big_kb = env_kb("EB200_GEMM_SMEM_BIG_KB", 100);    // when it fits one CTA per SM
   }
   return (total_ctas <= device_sm_count() ? big_kb : small_kb) * 1024;
 }
@@ -122,7 +124,8 @@ __device__ __forceinline__ float ld_global_f32(const float* p) {
 template <typename T, int MPAD, int EPI, bool XMC, bool W8>
 __global__ void __launch_bounds__(kGemmThreads, (MPAD >= 256 ? 1 : 2))
 skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmW2,
-                  const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXh, const GemmParams p, const int stages) {
+                  const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXh, const GemmParams p, const int stages,
+                  const __grid_constant__ L2Prefetch pf) {
   constexpr bool kDual = (EPI == EPI_SWIGLU);
   static_assert(!XMC || (MPAD == 64 && !kDual), "X multicast: 64-row tiles, single accumulator");
   static_assert(!W8 || (!XMC && !kDual), "W8A16: single weight stream, no X multicast");
@@ -203,6 +206,9 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
           ph ^= 1;
         }
       }
+      // every weight load of this CTA is issued: while the ring drains and the epilogue runs, stream this CTA's share of the
+      // next GEMM's leading weight tiles into L2
+      l2_prefetch_weights(pf, n_tile + static_cast<int>(gridDim.x) * split, static_cast<int>(gridDim.x * gridDim.y));
     }
   } else {
     // ===== MMA warpgroups =====
@@ -424,19 +430,19 @@ static bool xmc_enabled() {
 }
 template <typename T, int MPAD, int EPI, bool XMC, bool W8 = false>
 static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
-                        cudaStream_t s);
+                        cudaStream_t s, const L2Prefetch* pf);
 template <typename T, int MPAD, int EPI>
 static int launch_one(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const GemmParams& p, cudaStream_t s,
-                      const CUtensorMap* tmXh = nullptr) {
+                      const CUtensorMap* tmXh, const L2Prefetch* pf) {
   if constexpr (MPAD == 64 && EPI != EPI_SWIGLU) {
     const int tiles = (p.N + kBlockN - 1) / kBlockN;
-    if (tmXh && xmc_enabled() && tiles % 2 == 0 && 2 * p.splitk <= 8) return launch_one_x<T, MPAD, EPI, true>(tmW, tmW2, tmX, tmXh, p, s);
+    if (tmXh && xmc_enabled() && tiles % 2 == 0 && 2 * p.splitk <= 8) return launch_one_x<T, MPAD, EPI, true>(tmW, tmW2, tmX, tmXh, p, s, pf);
   }
-  return launch_one_x<T, MPAD, EPI, false>(tmW, tmW2, tmX, tmX, p, s);
+  return launch_one_x<T, MPAD, EPI, false>(tmW, tmW2, tmX, tmX, p, s, pf);
 }
 template <typename T, int MPAD, int EPI, bool XMC, bool W8>
 static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
-                        cudaStream_t s) {
+                        cudaStream_t s, const L2Prefetch* pf) {
   auto kern = skinny_gemm_wgmma<T, MPAD, EPI, XMC, W8>;
   dim3 grid((p.N + kBlockN - 1) / kBlockN, p.splitk);
   const int stages = stage_count_for(MPAD, EPI, static_cast<int>(grid.x * grid.y), W8);
@@ -454,20 +460,22 @@ static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const C
     if (e != cudaSuccess) return static_cast<int>(e);
     configured_dev[cur_dev] = true;
   }
+  L2Prefetch none;
+  memset(&none, 0, sizeof(none));
   return static_cast<int>(launch_kc(kern, grid, dim3(kGemmThreads), static_cast<size_t>(smem), s, dim3(XMC ? 2 : 1, p.splitk, 1), *tmW,
-                                    tmW2 ? *tmW2 : *tmW, *tmX, *tmXh, p, stages));
+                                    tmW2 ? *tmW2 : *tmW, *tmX, *tmXh, p, stages, pf ? *pf : none));
 }
 
 template <typename T, int MPAD>
 static int launch_epi(int epi, const CUtensorMap* a, const CUtensorMap* b, const CUtensorMap* c, const GemmParams& p,
-                      cudaStream_t s, const CUtensorMap* ch = nullptr) {
+                      cudaStream_t s, const CUtensorMap* ch, const L2Prefetch* pf) {
   switch (epi) {
-    case EPI_STORE: return launch_one<T, MPAD, EPI_STORE>(a, b, c, p, s, ch);
-    case EPI_RESIDUAL: return launch_one<T, MPAD, EPI_RESIDUAL>(a, b, c, p, s, ch);
-    case EPI_SWIGLU: return launch_one<T, MPAD, EPI_SWIGLU>(a, b, c, p, s, ch);
-    case EPI_QKV_ROPE: return launch_one<T, MPAD, EPI_QKV_ROPE>(a, b, c, p, s, ch);
-    case EPI_PARTIAL_F32: return launch_one<T, MPAD, EPI_PARTIAL_F32>(a, b, c, p, s, ch);
-    case EPI_SWIGLU_IL: return launch_one<T, MPAD, EPI_SWIGLU_IL>(a, b, c, p, s, ch);
+    case EPI_STORE: return launch_one<T, MPAD, EPI_STORE>(a, b, c, p, s, ch, pf);
+    case EPI_RESIDUAL: return launch_one<T, MPAD, EPI_RESIDUAL>(a, b, c, p, s, ch, pf);
+    case EPI_SWIGLU: return launch_one<T, MPAD, EPI_SWIGLU>(a, b, c, p, s, ch, pf);
+    case EPI_QKV_ROPE: return launch_one<T, MPAD, EPI_QKV_ROPE>(a, b, c, p, s, ch, pf);
+    case EPI_PARTIAL_F32: return launch_one<T, MPAD, EPI_PARTIAL_F32>(a, b, c, p, s, ch, pf);
+    case EPI_SWIGLU_IL: return launch_one<T, MPAD, EPI_SWIGLU_IL>(a, b, c, p, s, ch, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }
@@ -475,17 +483,17 @@ static int launch_epi(int epi, const CUtensorMap* a, const CUtensorMap* b, const
 // 256 activation rows per launch (prompt prefill: wgmma N = 256, the weights are streamed once per 256 prompt tokens instead of
 // once per 64): only the epilogues the target's decoder layer needs
 template <typename T>
-static int launch_epi256(int epi, const CUtensorMap* a, const CUtensorMap* c, const GemmParams& p, cudaStream_t s) {
+static int launch_epi256(int epi, const CUtensorMap* a, const CUtensorMap* c, const GemmParams& p, cudaStream_t s, const L2Prefetch* pf) {
   switch (epi) {
-    case EPI_RESIDUAL: return launch_one<T, 256, EPI_RESIDUAL>(a, nullptr, c, p, s);
-    case EPI_QKV_ROPE: return launch_one<T, 256, EPI_QKV_ROPE>(a, nullptr, c, p, s);
-    case EPI_SWIGLU_IL: return launch_one<T, 256, EPI_SWIGLU_IL>(a, nullptr, c, p, s);
+    case EPI_RESIDUAL: return launch_one<T, 256, EPI_RESIDUAL>(a, nullptr, c, p, s, nullptr, pf);
+    case EPI_QKV_ROPE: return launch_one<T, 256, EPI_QKV_ROPE>(a, nullptr, c, p, s, nullptr, pf);
+    case EPI_SWIGLU_IL: return launch_one<T, 256, EPI_SWIGLU_IL>(a, nullptr, c, p, s, nullptr, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }
 
 int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX,
-                const GemmParams& p_in, cudaStream_t s, const CUtensorMap* tmXh) {
+                const GemmParams& p_in, cudaStream_t s, const CUtensorMap* tmXh, const L2Prefetch* pf) {
   GemmParams p = p_in;
   if (p.splitk < 1 || p.m_rows > mpad) return static_cast<int>(cudaErrorInvalidValue);
   if (epi == EPI_SWIGLU || epi == EPI_SWIGLU_IL) {
@@ -493,32 +501,33 @@ int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUte
     if (!p.silu_lut) return static_cast<int>(cudaErrorNotReady);
   }
   if (dtype == DT_BF16) {
-    if (mpad == 16) return launch_epi<__nv_bfloat16, 16>(epi, tmW, tmW2, tmX, p, s);
-    if (mpad == 64) return launch_epi<__nv_bfloat16, 64>(epi, tmW, tmW2, tmX, p, s, tmXh);
-    if (mpad == 256) return launch_epi256<__nv_bfloat16>(epi, tmW, tmX, p, s);
+    if (mpad == 16) return launch_epi<__nv_bfloat16, 16>(epi, tmW, tmW2, tmX, p, s, nullptr, pf);
+    if (mpad == 64) return launch_epi<__nv_bfloat16, 64>(epi, tmW, tmW2, tmX, p, s, tmXh, pf);
+    if (mpad == 256) return launch_epi256<__nv_bfloat16>(epi, tmW, tmX, p, s, pf);
   } else if (dtype == DT_FP16) {
-    if (mpad == 16) return launch_epi<__half, 16>(epi, tmW, tmW2, tmX, p, s);
-    if (mpad == 64) return launch_epi<__half, 64>(epi, tmW, tmW2, tmX, p, s, tmXh);
-    if (mpad == 256) return launch_epi256<__half>(epi, tmW, tmX, p, s);
+    if (mpad == 16) return launch_epi<__half, 16>(epi, tmW, tmW2, tmX, p, s, nullptr, pf);
+    if (mpad == 64) return launch_epi<__half, 64>(epi, tmW, tmW2, tmX, p, s, tmXh, pf);
+    if (mpad == 256) return launch_epi256<__half>(epi, tmW, tmX, p, s, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }
 
 // W8A16: the epilogues of the target's decoder layer (+ EPI_STORE for mpad 16 / 64)
 template <typename T, int MPAD>
-static int launch_w8_epi(int epi, const CUtensorMap* w, const CUtensorMap* x, const GemmParams& p, cudaStream_t s) {
+static int launch_w8_epi(int epi, const CUtensorMap* w, const CUtensorMap* x, const GemmParams& p, cudaStream_t s, const L2Prefetch* pf) {
   switch (epi) {
     case EPI_STORE:
-      if constexpr (MPAD < 256) return launch_one_x<T, MPAD, EPI_STORE, false, true>(w, nullptr, x, x, p, s);
+      if constexpr (MPAD < 256) return launch_one_x<T, MPAD, EPI_STORE, false, true>(w, nullptr, x, x, p, s, pf);
       break;
-    case EPI_RESIDUAL: return launch_one_x<T, MPAD, EPI_RESIDUAL, false, true>(w, nullptr, x, x, p, s);
-    case EPI_QKV_ROPE: return launch_one_x<T, MPAD, EPI_QKV_ROPE, false, true>(w, nullptr, x, x, p, s);
-    case EPI_SWIGLU_IL: return launch_one_x<T, MPAD, EPI_SWIGLU_IL, false, true>(w, nullptr, x, x, p, s);
+    case EPI_RESIDUAL: return launch_one_x<T, MPAD, EPI_RESIDUAL, false, true>(w, nullptr, x, x, p, s, pf);
+    case EPI_QKV_ROPE: return launch_one_x<T, MPAD, EPI_QKV_ROPE, false, true>(w, nullptr, x, x, p, s, pf);
+    case EPI_SWIGLU_IL: return launch_one_x<T, MPAD, EPI_SWIGLU_IL, false, true>(w, nullptr, x, x, p, s, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }
 
-int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmX, const GemmParams& p_in, cudaStream_t s) {
+int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmX, const GemmParams& p_in, cudaStream_t s,
+                   const L2Prefetch* pf) {
   GemmParams p = p_in;
   if (p.splitk < 1 || p.m_rows > mpad || !p.w_scale) return static_cast<int>(cudaErrorInvalidValue);
   if (epi == EPI_SWIGLU_IL) {
@@ -526,13 +535,13 @@ int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const C
     if (!p.silu_lut) return static_cast<int>(cudaErrorNotReady);
   }
   if (dtype == DT_BF16) {
-    if (mpad == 16) return launch_w8_epi<__nv_bfloat16, 16>(epi, tmW, tmX, p, s);
-    if (mpad == 64) return launch_w8_epi<__nv_bfloat16, 64>(epi, tmW, tmX, p, s);
-    if (mpad == 256) return launch_w8_epi<__nv_bfloat16, 256>(epi, tmW, tmX, p, s);
+    if (mpad == 16) return launch_w8_epi<__nv_bfloat16, 16>(epi, tmW, tmX, p, s, pf);
+    if (mpad == 64) return launch_w8_epi<__nv_bfloat16, 64>(epi, tmW, tmX, p, s, pf);
+    if (mpad == 256) return launch_w8_epi<__nv_bfloat16, 256>(epi, tmW, tmX, p, s, pf);
   } else if (dtype == DT_FP16) {
-    if (mpad == 16) return launch_w8_epi<__half, 16>(epi, tmW, tmX, p, s);
-    if (mpad == 64) return launch_w8_epi<__half, 64>(epi, tmW, tmX, p, s);
-    if (mpad == 256) return launch_w8_epi<__half, 256>(epi, tmW, tmX, p, s);
+    if (mpad == 16) return launch_w8_epi<__half, 16>(epi, tmW, tmX, p, s, pf);
+    if (mpad == 64) return launch_w8_epi<__half, 64>(epi, tmW, tmX, p, s, pf);
+    if (mpad == 256) return launch_w8_epi<__half, 256>(epi, tmW, tmX, p, s, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }

@@ -85,16 +85,30 @@ struct GemmParams {
   const float* w_scale;
 };
 
+// L2 prefetch of the weight tiles a later skinny_gemm_wgmma launch reads first.  Weights depend on no kernel, so a kernel that
+// leaves HBM idle (attention, RMSNorm, a GEMM's drain) can fetch them before its griddepcontrol.wait.  That GEMM runs the grid
+// n_tiles x splitk over num_kb k-blocks; split s reads k-blocks [kb_begin(s), kb_end(s)) in order.  The plan covers k-block
+// kb_begin(s) + j of every (n-tile, split) for j in [j0, j1): all CTAs of that GEMM are resident at once, so j-major is the
+// order in which it consumes them.  j1 <= j0 prefetches nothing.  Host side: l2_plan in engine.cu.
+struct alignas(64) L2Prefetch {
+  CUtensorMap tm;  // the weight's map (box 128 rows x 64 K-elements, as the GEMM loads it)
+  int n_tiles, splitk, num_kb;
+  int j0, j1;
+};
+
 // Returns cudaError_t-compatible int (0 = ok).  mpad in {16, 64}.  tm* are HOST pointers to encoded maps.
+// pf (optional): after its last weight load, the producer lane of every CTA prefetches its share of that plan (the GEMM that
+// follows), so HBM keeps streaming while this launch drains (cluster reduction, epilogue) and the next kernels ramp.
 // tmXh (optional, mpad == 64): the same activation buffer with a 32-row box -- enables the X-multicast variant (neighbouring n-tiles
 // in a cluster share every X tile, each CTA loads half of it)
 int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX,
-                const GemmParams& p, cudaStream_t s, const CUtensorMap* tmXh = nullptr);
+                const GemmParams& p, cudaStream_t s, const CUtensorMap* tmXh = nullptr, const L2Prefetch* pf = nullptr);
 // W8A16 form of launch_gemm: tmW maps an int8 [N][K] weight (make_tmap_w8 layout: box 128 rows x 64 bytes, no swizzle) and
 // p.w_scale its row scales.  The kernel forms W' = T((q * scale) * kInv127) in shared memory and runs the same wgmma sequence and
 // epilogue as launch_gemm, so the result is bit-identical to launch_gemm on W'.  mpad 16 / 64: EPI_STORE, EPI_RESIDUAL,
 // EPI_QKV_ROPE, EPI_SWIGLU_IL; mpad 256: the last three.
-int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmX, const GemmParams& p, cudaStream_t s);
+int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmX, const GemmParams& p, cudaStream_t s,
+                   const L2Prefetch* pf = nullptr);
 // bring-up / debugging aid: same epilogues, plain FMA main loop, no TMA/wgmma.  W/W2/X are raw pointers.
 int launch_gemm_simt(int dtype, int mpad, int epi, const void* W, const void* W2, const void* X, long ldx,
                      const GemmParams& p, cudaStream_t s);
@@ -227,13 +241,14 @@ bool chain_phase_ok(int N, int K, int fin);
 // elementwise / reduction kernels (misc.cu)
 // ----------------------------------------------------------------------------------------------
 // y[m, col_off : col_off+H] = w * T(x_row * rsqrt(mean(x_row^2) + eps));  x_row = src[row_ids ? row_ids[m] : m]
+// pf (optional, also for launch_e3_input): weight tiles of the GEMM that follows, prefetched into L2 at kernel start
 int launch_rmsnorm(int dtype, const void* src, long ld_src, const int64_t* row_ids64, const int* row_ids32,
-                   const void* w, void* y, long ld_y, int col_off, int H, float eps, int rows, cudaStream_t s);
+                   const void* w, void* y, long ld_y, int col_off, int H, float eps, int rows, cudaStream_t s, const L2Prefetch* pf = nullptr);
 // EAGLE-3 draft input: cat[m] = (w_emb * norm(table[ids[m]]), w_hid * norm(h_m)) with h_m = hsrc[src_rows ? src_rows[m] : m]
 // (src_rows: also copies h_m to hdst[m])
 int launch_e3_input(int dtype, const void* table, long ld_table, const int64_t* ids64, const int* ids32, const void* w_emb, const void* hsrc,
                     long ld_hsrc, const int* src_rows, void* hdst, long ld_hdst, const void* w_hid, void* cat, long ld_cat, int H, float eps,
-                    int rows, cudaStream_t s);
+                    int rows, cudaStream_t s, const L2Prefetch* pf = nullptr);
 // dst[m, col_off: col_off+H] = table[ids[m]]
 int launch_gather_rows(int dtype, const void* table, long ld_table, const int64_t* ids64, const int* ids32, void* dst,
                        long ld_dst, int col_off, int H, int rows, cudaStream_t s);
@@ -276,10 +291,9 @@ struct AttnParams {
   const uint64_t* mask; // [rows][2] ancestor bits over the tree columns; nullptr => causal (row r sees columns 0..r)
   int max_kv;           // capacity used to size shared memory (n_ctx + n_tree <= max_kv)
   unsigned long long* trace;  // optional (EB200_ATTN_TRACE): [n_ctas][16] %globaltimer stamps of thread 0 at the phase boundaries
-  // optional: weight bytes the NEXT kernel (the layer's chain launch) streams first; every CTA asks L2 to prefetch its share at
-  // kernel start (cp.async.bulk.prefetch.L2), so HBM keeps streaming while this latency-bound kernel runs
-  const void* pf_ptr[2];
-  unsigned long long pf_bytes[2];
+  // optional (host pointer): weight tiles of the GEMM that follows; every CTA prefetches its share into L2 at kernel start, so
+  // HBM keeps streaming while this latency-bound kernel runs
+  const L2Prefetch* pf;
 };
 int launch_attention(int dtype, const AttnParams& p, cudaStream_t s);
 

@@ -178,11 +178,6 @@ __device__ __forceinline__ void cursor_advance(UnitCursor& c, const ChainArgs& a
     cursor_enter_phase(c, args, cta, G);
   }
 }
-__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1)
-               : "memory");
-}
-
 // per-tile contributor table (shared memory): CTAs [c_first, c_last] hold partials of tile t; the first one at slot
 // slot_first, every later one at slot 0 (its range starts inside the tile)
 struct TileSrc {

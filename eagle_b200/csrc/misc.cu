@@ -31,8 +31,9 @@ template <typename T>
 __global__ void __launch_bounds__(256) rmsnorm_kernel(const T* __restrict__ src, long ld_src,
                                                       const int64_t* __restrict__ ids64, const int* __restrict__ ids32,
                                                       const T* __restrict__ w, T* __restrict__ y, long ld_y, int col_off,
-                                                      int H, float eps) {
+                                                      int H, float eps, const __grid_constant__ L2Prefetch pf) {
   pdl_launch_dependents();
+  if (threadIdx.x < 32) l2_prefetch_weights(pf, blockIdx.x * 32 + threadIdx.x, gridDim.x * 32);  // weights: no dependency wait
   pdl_wait();
   using D = DT<T>;
   __shared__ float red[32];
@@ -69,16 +70,18 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const T* __restrict__ src,
 }
 
 int launch_rmsnorm(int dtype, const void* src, long ld_src, const int64_t* ids64, const int* ids32, const void* w, void* y,
-                   long ld_y, int col_off, int H, float eps, int rows, cudaStream_t s) {
+                   long ld_y, int col_off, int H, float eps, int rows, cudaStream_t s, const L2Prefetch* pf) {
   if (H % 8 || rows <= 0) return static_cast<int>(cudaErrorInvalidValue);
+  L2Prefetch none;
+  memset(&none, 0, sizeof(none));
   if (dtype == DT_BF16)
     launch_k(rmsnorm_kernel<__nv_bfloat16>, dim3(rows), dim3(256), 0, s, 1, reinterpret_cast<const __nv_bfloat16*>(src), ld_src, ids64, ids32,
                                                         reinterpret_cast<const __nv_bfloat16*>(w),
-                                                        reinterpret_cast<__nv_bfloat16*>(y), ld_y, col_off, H, eps);
+                                                        reinterpret_cast<__nv_bfloat16*>(y), ld_y, col_off, H, eps, pf ? *pf : none);
   else
     launch_k(rmsnorm_kernel<__half>, dim3(rows), dim3(256), 0, s, 1, reinterpret_cast<const __half*>(src), ld_src, ids64, ids32,
                                                  reinterpret_cast<const __half*>(w), reinterpret_cast<__half*>(y), ld_y,
-                                                 col_off, H, eps);
+                                                 col_off, H, eps, pf ? *pf : none);
   return static_cast<int>(cudaGetLastError());
 }
 
@@ -91,8 +94,13 @@ int launch_rmsnorm(int dtype, const void* src, long ld_src, const int64_t* ids64
 template <typename T>
 __global__ void __launch_bounds__(256) e3_input_kernel(const T* table, long ld_table, const int64_t* ids64, const int* ids32, const T* w_emb,
                                                        const T* hsrc, long ld_hsrc, const int* src_rows, T* hdst, long ld_hdst,
-                                                       const T* w_hid, T* cat, long ld_cat, int H, float eps) {
+                                                       const T* w_hid, T* cat, long ld_cat, int H, float eps,
+                                                       const __grid_constant__ L2Prefetch pf) {
   pdl_launch_dependents();
+  if (threadIdx.x < 32) {  // weights: no dependency wait
+    const int cta = blockIdx.x + gridDim.x * blockIdx.y;
+    l2_prefetch_weights(pf, cta * 32 + threadIdx.x, gridDim.x * gridDim.y * 32);
+  }
   pdl_wait();
   using D = DT<T>;
   __shared__ float red[32];
@@ -148,19 +156,21 @@ __global__ void __launch_bounds__(256) e3_input_kernel(const T* table, long ld_t
 
 int launch_e3_input(int dtype, const void* table, long ld_table, const int64_t* ids64, const int* ids32, const void* w_emb, const void* hsrc,
                     long ld_hsrc, const int* src_rows, void* hdst, long ld_hdst, const void* w_hid, void* cat, long ld_cat, int H, float eps,
-                    int rows, cudaStream_t s) {
+                    int rows, cudaStream_t s, const L2Prefetch* pf) {
   if (H % 8 || rows <= 0 || ld_table % 8 || ld_hsrc % 8 || ld_hdst % 8 || ld_cat % 8) return static_cast<int>(cudaErrorInvalidValue);
   if (src_rows && hsrc == hdst) return static_cast<int>(cudaErrorInvalidValue);  // a gather must not alias its destination
+  L2Prefetch none;
+  memset(&none, 0, sizeof(none));
   if (dtype == DT_BF16) {
     using T = __nv_bfloat16;
     launch_k(e3_input_kernel<T>, dim3(rows, 2), dim3(256), 0, s, 1, reinterpret_cast<const T*>(table), ld_table, ids64, ids32,
              reinterpret_cast<const T*>(w_emb), reinterpret_cast<const T*>(hsrc), ld_hsrc, src_rows, reinterpret_cast<T*>(hdst), ld_hdst,
-             reinterpret_cast<const T*>(w_hid), reinterpret_cast<T*>(cat), ld_cat, H, eps);
+             reinterpret_cast<const T*>(w_hid), reinterpret_cast<T*>(cat), ld_cat, H, eps, pf ? *pf : none);
   } else {
     using T = __half;
     launch_k(e3_input_kernel<T>, dim3(rows, 2), dim3(256), 0, s, 1, reinterpret_cast<const T*>(table), ld_table, ids64, ids32,
              reinterpret_cast<const T*>(w_emb), reinterpret_cast<const T*>(hsrc), ld_hsrc, src_rows, reinterpret_cast<T*>(hdst), ld_hdst,
-             reinterpret_cast<const T*>(w_hid), reinterpret_cast<T*>(cat), ld_cat, H, eps);
+             reinterpret_cast<const T*>(w_hid), reinterpret_cast<T*>(cat), ld_cat, H, eps, pf ? *pf : none);
   }
   return static_cast<int>(cudaGetLastError());
 }

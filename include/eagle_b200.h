@@ -220,6 +220,13 @@ int eb200_k_chain_gemm(int32_t dtype, int32_t mode, const void* W, const void* X
 int eb200_k_gemm_bench(int32_t dtype, int32_t epilogue, int32_t M, int32_t N, int32_t K, int32_t splitk, int32_t n_weights,
                        int32_t iters, int32_t use_graph, double* us_per_launch);
 int eb200_k_rmsnorm(int32_t dtype, const void* x, const void* w, void* y, int32_t rows, int32_t H, float eps, void* stream);
+/* a kernel that also prefetches another GEMM's weight into L2; its outputs must equal the kernel's own.  kernel 0: the cluster
+ * GEMM of eb200_k_gemm (epilogue 0 store / 1 residual, W [N, K], X, out, res, M, splitk); kernel 1: eb200_k_rmsnorm (W = the
+ * norm weight [N], X = x [M, N], eps).  The prefetched weight is P [PN, PK] (model dtype) under the grid (PN / 128 tiles x
+ * p_splitk): k-block rows [j0, j1) of every (tile, split), passed unclipped to the device. */
+int eb200_k_prefetch(int32_t dtype, int32_t kernel, int32_t epilogue, const void* W, const void* X, void* out, const void* res, int32_t M,
+                     int32_t N, int32_t K, int32_t splitk, float eps, const void* P, int32_t PN, int32_t PK, int32_t p_splitk, int32_t j0,
+                     int32_t j1, void* stream);
 int eb200_k_attention(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, void* out, int32_t rows,
                       int32_t n_heads, int32_t n_kv_heads, int64_t kv_cap, int32_t n_ctx, int32_t n_tree,
                       const uint64_t* mask, void* stream);
