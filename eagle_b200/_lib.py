@@ -97,6 +97,10 @@ SIGNATURES = {
     "eb200_k_rmsnorm": (_I32, [_I32, _P, _P, _P, _I32, _I32, C.c_float, _P]),
     "eb200_k_prefetch": (_I32, [_I32, _I32, _I32, _P, _P, _P, _P, _I32, _I32, _I32, _I32, C.c_float, _P, _I32, _I32, _I32, _I32, _I32, _P]),
     "eb200_k_attention": (_I32, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _I64, _I32, _I32, _P, _P]),
+    "eb200_k_attention_plan": (_I32, [_I32, _I32, _I32, _I32, _I32, C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I32),
+                                      C.POINTER(_I64)]),
+    "eb200_k_attention_ex": (_I32, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _I64, _I32, _P, _I32, _I32, _I32, _I32, _P, _I32,
+                                    _I32, _P]),
     "eb200_k_qkv_rope": (_I32, [_I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I64, _I32, _I32, _P]),
     "eb200_k_argmax": (_I32, [_I32, _P, _I32, _I32, _P, _P]),
     "eb200_k_logsoftmax_topk": (_I32, [_I32, _P, _I32, _I32, _I32, _P, _P, _P]),

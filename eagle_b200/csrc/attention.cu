@@ -512,24 +512,28 @@ template <typename T, int HPC> static int launch_hpc(const AttnParams& p, int kv
   return static_cast<int>(launch_kc(kern, grid, dim3(kThreads), smem, s, dim3(1, 1, kvs), *p.tmK, *p.tmV, p, kv_stride, kvs, p.pf ? *p.pf : none));
 }
 
-int launch_attention(int dtype, const AttnParams& p, cudaStream_t s) {
-  if (p.rows <= 0 || p.n_tree > 128 || p.n_heads % p.n_kv_heads || p.max_kv < 1 || !p.tmK || !p.tmV) return static_cast<int>(cudaErrorInvalidValue);
-  static int max_hpc = 0, max_kvs = 0;
-  if (!max_hpc) {
+int attention_geometry(int max_kv, int n_heads, int n_kv_heads, int hpc_cap, int kvs_cap, AttnGeometry* g) {
+  auto cap_ok = [](int v) { return v == 0 || v == 1 || v == 2 || v == 4; };
+  if (max_kv < 1 || n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads || !cap_ok(hpc_cap) || !cap_ok(kvs_cap))
+    return static_cast<int>(cudaErrorInvalidValue);
+  static int env_hpc = 0, env_kvs = 0;
+  if (!env_hpc) {
     const char* e = getenv("EB200_ATTN_HPC");  // tuning knobs: cap on query heads per CTA, cap on the KV split
-    max_hpc = e ? atoi(e) : 2;
-    if (max_hpc != 1 && max_hpc != 2 && max_hpc != 4) max_hpc = 2;
+    env_hpc = e ? atoi(e) : 2;
+    if (env_hpc != 1 && env_hpc != 2 && env_hpc != 4) env_hpc = 2;
     const char* k = getenv("EB200_ATTN_KVS");
-    max_kvs = k ? atoi(k) : 4;
-    if (max_kvs != 1 && max_kvs != 2 && max_kvs != 4) max_kvs = 4;
+    env_kvs = k ? atoi(k) : 4;
+    if (env_kvs != 1 && env_kvs != 2 && env_kvs != 4) env_kvs = 4;
   }
+  const int max_hpc = hpc_cap ? hpc_cap : env_hpc;
+  const int max_kvs = kvs_cap ? kvs_cap : env_kvs;
   // KV split over a cluster: aim at ~3 tiles (192 KV rows) per CTA
-  const int tiles_all = (p.max_kv + kKvTile - 1) / kKvTile;
+  const int tiles_all = (max_kv + kKvTile - 1) / kKvTile;
   int kvs = 1;
   while (kvs < max_kvs && tiles_all > 3 * kvs) kvs *= 2;
   const int tiles_per = (tiles_all + kvs - 1) / kvs;
   const int kv_stride = tiles_per * kKvTile + 8;
-  const int n_rep = p.n_heads / p.n_kv_heads;
+  const int n_rep = n_heads / n_kv_heads;
   // most heads per CTA (fewest K/V re-reads) whose score strip still fits in shared memory
   int hpc = 1;
   const size_t limit = 220 * 1024;
@@ -537,6 +541,28 @@ int launch_attention(int dtype, const AttnParams& p, cudaStream_t s) {
   else if (max_hpc >= 2 && n_rep % 2 == 0 && attn_smem(2, kv_stride) <= limit) hpc = 2;
   const size_t smem = attn_smem(hpc, kv_stride);
   if (smem > limit) return static_cast<int>(cudaErrorInvalidValue);
+  g->hpc = hpc;
+  g->kvs = kvs;
+  g->kv_stride = kv_stride;
+  g->smem = smem;
+  return 0;
+}
+
+int attention_max_kv() {
+  // one head per CTA and the widest KV split the policy allows: the smallest score strip for a given max_kv
+  AttnGeometry g;
+  int best = 0;
+  for (int tiles = 1; attention_geometry(tiles * kKvTile, 1, 1, 0, 0, &g) == 0; ++tiles) best = tiles * kKvTile;
+  return best;
+}
+
+int launch_attention(int dtype, const AttnParams& p, cudaStream_t s) {
+  if (p.rows <= 0 || p.n_tree > 128 || !p.tmK || !p.tmV) return static_cast<int>(cudaErrorInvalidValue);
+  AttnGeometry geo;
+  const int rc = attention_geometry(p.max_kv, p.n_heads, p.n_kv_heads, p.hpc_cap, p.kvs_cap, &geo);
+  if (rc) return rc;
+  const int hpc = geo.hpc, kvs = geo.kvs, kv_stride = geo.kv_stride;
+  const size_t smem = geo.smem;
   if (dtype == DT_BF16) {
     if (hpc == 4) return launch_hpc<__nv_bfloat16, 4>(p, kv_stride, kvs, smem, s);
     if (hpc == 2) return launch_hpc<__nv_bfloat16, 2>(p, kv_stride, kvs, smem, s);

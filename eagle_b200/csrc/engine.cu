@@ -321,6 +321,14 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
   if (c.depth < 1 || c.depth + 2 > 16) return fail("depth must be in [1, 14]");
   if (c.top_k * (c.depth) > 128) return fail("depth * top_k must be <= 128 (draft tree columns)");
   if (c.top_k + c.depth * c.top_k * c.top_k < c.total_token - 1) return fail("candidate pool smaller than total_token - 1");
+  {
+    // the draft planes hold max_length + 128 + depth * top_k rows, and the attention score strip must be able to span them all
+    const long dcap = static_cast<long>(c.max_length) + 64 + c.depth * c.top_k + 64;
+    const int lim = attention_max_kv();
+    if (dcap > lim)
+      return fail("max_length %d too large: the draft KV needs %ld rows, tree attention holds at most %d (max_length <= %d at "
+                  "depth %d, top_k %d)", c.max_length, dcap, lim, lim - 128 - c.depth * c.top_k, c.depth, c.top_k);
+  }
   int dev_count = 0;
   CK(cudaGetDeviceCount(&dev_count));
   if (dev_count == 0) return fail("no CUDA device: eagle_b200 has no CPU path");
@@ -3042,6 +3050,30 @@ extern "C" int eb200_k_rmsnorm(int32_t dtype, const void* x, const void* w, void
 extern "C" int eb200_k_attention(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, void* out, int32_t rows,
                                  int32_t n_heads, int32_t n_kv_heads, int64_t kv_cap, int32_t n_ctx, int32_t n_tree,
                                  const uint64_t* mask, void* stream) {
+  return eb200_k_attention_ex(dtype, q, k_cache, v_cache, out, rows, n_heads, n_kv_heads, kv_cap, n_ctx + n_tree, nullptr, -1, -1,
+                              n_ctx, n_tree, mask, 0, 0, stream);
+}
+
+extern "C" int eb200_k_attention_plan(int32_t max_kv, int32_t n_heads, int32_t n_kv_heads, int32_t hpc_cap, int32_t kvs_cap,
+                                      int32_t* hpc, int32_t* kvs, int32_t* kv_stride, int64_t* smem) {
+  AttnGeometry g;
+  if (attention_geometry(max_kv, n_heads, n_kv_heads, hpc_cap, kvs_cap, &g))
+    return fail("attention: no launch geometry for max_kv %d, %d / %d heads, caps hpc %d kvs %d (max_kv <= %d under the default "
+                "caps; caps must be 0, 1, 2 or 4)", max_kv, n_heads, n_kv_heads, hpc_cap, kvs_cap, attention_max_kv());
+  if (hpc) *hpc = g.hpc;
+  if (kvs) *kvs = g.kvs;
+  if (kv_stride) *kv_stride = g.kv_stride;
+  if (smem) *smem = static_cast<int64_t>(g.smem);
+  return 0;
+}
+
+extern "C" int eb200_k_attention_ex(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, void* out, int32_t rows,
+                                    int32_t n_heads, int32_t n_kv_heads, int64_t kv_cap, int32_t max_kv, const int32_t* st,
+                                    int32_t rows_idx, int32_t n_ctx_idx, int32_t n_ctx_add, int32_t n_tree, const uint64_t* mask,
+                                    int32_t hpc_cap, int32_t kvs_cap, void* stream) {
+  TRY(eb200_k_attention_plan(max_kv, n_heads, n_kv_heads, hpc_cap, kvs_cap, nullptr, nullptr, nullptr, nullptr));
+  if (rows < 1 || n_tree < 0 || n_tree > 128) return fail("eb200_k_attention_ex: rows must be >= 1 and n_tree in [0, 128]");
+  if ((rows_idx >= 0 || n_ctx_idx >= 0) && !st) return fail("eb200_k_attention_ex: a state index needs the state pointer");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   AttnParams a;
   memset(&a, 0, sizeof(a));
@@ -3054,12 +3086,14 @@ extern "C" int eb200_k_attention(int32_t dtype, const void* q, const void* k_cac
   a.n_heads = n_heads;
   a.n_kv_heads = n_kv_heads;
   a.rows = rows;
-  a.rows_idx = -1;
-  a.st = nullptr;
-  a.n_ctx = DynInt{-1, n_ctx};
+  a.rows_idx = rows_idx;
+  a.st = st;
+  a.n_ctx = DynInt{n_ctx_idx, n_ctx_add};
   a.n_tree = n_tree;
   a.mask = mask;
-  a.max_kv = n_ctx + n_tree;
+  a.max_kv = max_kv;
+  a.hpc_cap = hpc_cap;
+  a.kvs_cap = kvs_cap;
   CUtensorMap mk, mv;
   TRY(make_tmap(&mk, dtype, k_cache, static_cast<uint64_t>(n_kv_heads) * kv_cap, 128, 64));
   TRY(make_tmap(&mv, dtype, v_cache, static_cast<uint64_t>(n_kv_heads) * kv_cap, 128, 64));

@@ -294,7 +294,19 @@ struct AttnParams {
   // optional (host pointer): weight tiles of the GEMM that follows; every CTA prefetches its share into L2 at kernel start, so
   // HBM keeps streaming while this latency-bound kernel runs
   const L2Prefetch* pf;
+  // caps on the query heads per CTA and on the KV split, each 1, 2 or 4; 0 = the EB200_ATTN_HPC / EB200_ATTN_KVS policy
+  int hpc_cap, kvs_cap;
 };
+// Launch geometry of the attention kernel for a score strip of max_kv columns: HPC query heads of one kv head per CTA, a KV
+// split over a cluster of KVS CTAs (each holds kv_stride strip columns per row) and the dynamic shared memory.  Host only.
+struct AttnGeometry {
+  int hpc, kvs, kv_stride;
+  size_t smem;
+};
+// 0, or cudaErrorInvalidValue when a cap is not 0/1/2/4 or the strip does not fit in shared memory
+int attention_geometry(int max_kv, int n_heads, int n_kv_heads, int hpc_cap, int kvs_cap, AttnGeometry* g);
+// largest max_kv the kernel accepts under the default caps (16896 with EB200_ATTN_KVS unset)
+int attention_max_kv();
 int launch_attention(int dtype, const AttnParams& p, cudaStream_t s);
 
 // ----------------------------------------------------------------------------------------------

@@ -230,6 +230,19 @@ int eb200_k_prefetch(int32_t dtype, int32_t kernel, int32_t epilogue, const void
 int eb200_k_attention(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, void* out, int32_t rows,
                       int32_t n_heads, int32_t n_kv_heads, int64_t kv_cap, int32_t n_ctx, int32_t n_tree,
                       const uint64_t* mask, void* stream);
+/* host only, no kernel: the tree attention's launch geometry for a score strip of max_kv columns -- query heads per CTA
+ * (hpc), KV split over a cluster (kvs), strip columns per CTA row (kv_stride) and dynamic shared memory in bytes.  hpc_cap /
+ * kvs_cap: 1, 2 or 4 caps the choice, 0 keeps the engine's policy (EB200_ATTN_HPC / EB200_ATTN_KVS, default 2 / 4).  Fails
+ * with a message when max_kv exceeds what shared memory holds (16896 under the default caps). */
+int eb200_k_attention_plan(int32_t max_kv, int32_t n_heads, int32_t n_kv_heads, int32_t hpc_cap, int32_t kvs_cap, int32_t* hpc,
+                           int32_t* kvs, int32_t* kv_stride, int64_t* smem);
+/* eb200_k_attention as the engine launches it: the strip is sized for max_kv columns (kv_len = min(n_ctx + n_tree, max_kv));
+ * st (device int32, may be null) supplies the valid row count min(rows, st[rows_idx]) when rows_idx >= 0 and
+ * n_ctx = st[n_ctx_idx] + n_ctx_add (n_ctx_add alone when n_ctx_idx < 0); caps as in eb200_k_attention_plan. */
+int eb200_k_attention_ex(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, void* out, int32_t rows,
+                         int32_t n_heads, int32_t n_kv_heads, int64_t kv_cap, int32_t max_kv, const int32_t* st, int32_t rows_idx,
+                         int32_t n_ctx_idx, int32_t n_ctx_add, int32_t n_tree, const uint64_t* mask, int32_t hpc_cap,
+                         int32_t kvs_cap, void* stream);
 int eb200_k_qkv_rope(int32_t dtype, int32_t simt, const void* Wqkv, const void* X, void* q_out, void* k_cache,
                      void* v_cache, const void* cos, const void* sin, const int32_t* pos, int32_t M, int32_t n_heads,
                      int32_t n_kv_heads, int32_t K, int64_t kv_cap, int32_t kv_base, int32_t splitk, void* stream);
