@@ -107,6 +107,7 @@ SIGNATURES = {
     "eb200_k_topk_raw": (_I32, [_I32, _P, _I32, _I32, _I32, _P, _P, _P]),
     "eb200_k_generate_candidates": (_I32, [_P, _I32, _I32, _P, _I32, _P, _I32, _I32, _P]),
     "eb200_k_tree_finalize": (_I32, [_I32, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, C.POINTER(_I32), C.POINTER(_I32)]),
+    "eb200_k_tree_grow": (_I32, [_I32, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "eb200_k_sample_posterior": (_I32, [_I32, _P, _I32, _P, _P, _I32, _I32, _I32, C.c_float, C.c_float, _I32, _P, _I32,
                                          C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I32)]),
     "eb200_k_greedy_accept": (_I32, [_P, _P, _P, _I32, _I32, _I32, C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I32)]),

@@ -3218,6 +3218,65 @@ extern "C" int eb200_k_tree_finalize(int32_t dtype, const float* scores, const i
   return 0;
 }
 
+// draft-tree growth on host-supplied per-level top-k tables: tree_seed then tree_expand for level 0..depth-1, the frontier
+// copied out after the seed and after every level.  The tables do not depend on what the kernels produce, so a plain
+// transcription of cnets.py:703-757 driven by the same tables must give the same integers and the same rounded scores.
+extern "C" int eb200_k_tree_grow(int32_t dtype, const float* topk_p, const int32_t* topk_i, const int64_t* d2t, int32_t d2t_len,
+                                 int32_t k, int32_t depth, int32_t last_row, float* scores, int32_t* tokens, int32_t* parents,
+                                 int32_t* front_ids, int32_t* front_src, int32_t* front_cs, float* front_scores,
+                                 uint64_t* front_mask) {
+  if (dtype != EB200_BF16 && dtype != EB200_FP16) return fail("eb200_k_tree_grow: dtype must be bf16 or fp16");
+  if (!topk_p || !topk_i) return fail("eb200_k_tree_grow: null top-k table");
+  if (k < 1 || k > 32) return fail("eb200_k_tree_grow: top_k must be in [1, 32]");
+  if (depth < 1 || depth + 2 > 16) return fail("eb200_k_tree_grow: depth must be in [1, 14]");
+  if (depth * k > 128) return fail("eb200_k_tree_grow: depth * top_k must be <= 128 (draft tree columns)");
+  if (last_row < 0) return fail("eb200_k_tree_grow: last_row must be >= 0");
+  if (d2t && d2t_len < 1) return fail("eb200_k_tree_grow: empty d2t");
+  const int kk = k * k, pool = k + depth * kk, rows = 1 + depth * k;
+  for (int i = 0; i < rows * k; ++i) {
+    if (topk_i[i] < 0 || (d2t && topk_i[i] >= d2t_len)) return fail("eb200_k_tree_grow: top-k index %d out of range at %d", topk_i[i], i);
+  }
+  Scratch sc;
+  TreeBuffers tb;
+  memset(&tb, 0, sizeof(tb));
+  tb.scores = sc.get<float>(pool);
+  tb.tokens = sc.get<int>(pool);
+  tb.parents = sc.get<int>(rows);
+  tb.front_scores = sc.get<float>(k);
+  tb.front_ids = sc.get<int>(k);
+  tb.front_src = sc.get<int>(k);
+  tb.front_cs = sc.get<int>(k);
+  tb.front_mask = sc.get<uint64_t>(2 * k);
+  int* st = sc.get<int>(S_COUNT);
+  float* d_p = sc.get<float>(rows * k);
+  int* d_i = sc.get<int>(rows * k);
+  int64_t* d_d2t = d2t ? sc.get<int64_t>(d2t_len) : nullptr;
+  if (!d_i || (d2t && !d_d2t)) return fail("scratch allocation failed");
+  CK(cudaMemcpy(d_p, topk_p, rows * k * sizeof(float), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(d_i, topk_i, rows * k * sizeof(int), cudaMemcpyHostToDevice));
+  if (d2t) CK(cudaMemcpy(d_d2t, d2t, d2t_len * sizeof(int64_t), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(st + S_LASTROW, &last_row, sizeof(int), cudaMemcpyHostToDevice));
+  auto snapshot = [&](int slot) -> int {
+    CK(cudaDeviceSynchronize());
+    if (front_ids) CK(cudaMemcpy(front_ids + slot * k, tb.front_ids, k * sizeof(int), cudaMemcpyDeviceToHost));
+    if (front_src) CK(cudaMemcpy(front_src + slot * k, tb.front_src, k * sizeof(int), cudaMemcpyDeviceToHost));
+    if (front_cs) CK(cudaMemcpy(front_cs + slot * k, tb.front_cs, k * sizeof(int), cudaMemcpyDeviceToHost));
+    if (front_scores) CK(cudaMemcpy(front_scores + slot * k, tb.front_scores, k * sizeof(float), cudaMemcpyDeviceToHost));
+    if (front_mask) CK(cudaMemcpy(front_mask + slot * 2 * k, tb.front_mask, 2 * k * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    return 0;
+  };
+  CKL(launch_tree_seed(d_p, d_i, d_d2t, k, tb, st, 0));
+  TRY(snapshot(0));
+  for (int level = 0; level < depth; ++level) {
+    CKL(launch_tree_expand(dtype, d_p + (1 + level * k) * k, d_i + (1 + level * k) * k, d_d2t, k, level, tb, 0));
+    TRY(snapshot(level + 1));
+  }
+  if (scores) CK(cudaMemcpy(scores, tb.scores, pool * sizeof(float), cudaMemcpyDeviceToHost));
+  if (tokens) CK(cudaMemcpy(tokens, tb.tokens, pool * sizeof(int), cudaMemcpyDeviceToHost));
+  if (parents) CK(cudaMemcpy(parents, tb.parents, rows * sizeof(int), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 extern "C" int eb200_k_greedy_accept(const int32_t* node_argmax, const int32_t* draft_tokens, const int32_t* retrieve, int32_t T,
                                      int32_t n_leaf, int32_t max_depth, int32_t* best, int32_t* accept_length, int32_t* bonus) {
   if (T < 1 || T > 128 || max_depth > 16 || n_leaf > 128) return fail("eb200_k_greedy_accept: bad arguments");

@@ -45,16 +45,21 @@ int launch_tree_seed(const float* topk_p, const int* topk_i, const int64_t* d2t,
 // --------------------------------------------------------------------------------------------------------------
 // level expansion: cnets.py:728-757.  One CTA, one thread per (frontier slot j, child c).
 // --------------------------------------------------------------------------------------------------------------
+constexpr int kExpandMaxK = 32;  // largest top_k of tree_expand_kernel: k * k candidates, one per thread of a 1024-thread CTA
+static_assert(kExpandMaxK * kExpandMaxK <= 1024, "tree_expand_kernel runs one thread per candidate in a single CTA");
+
 template <typename T>
 __global__ void __launch_bounds__(1024) tree_expand_kernel(const float* __restrict__ topk_p, const int* __restrict__ topk_i,
                                                            const int64_t* __restrict__ d2t, int k, int level,
                                                            TreeBuffers tb) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ float cu[1024];
-  __shared__ int tok[1024];
-  __shared__ uint64_t old_mask[64];
-  __shared__ int new_cs[32];
+  // one thread per candidate and two mask words per frontier slot: all four arrays are sized by kExpandMaxK, the bound
+  // launch_tree_expand enforces (eb200_create accepts top_k <= 16, well inside it)
+  __shared__ float cu[kExpandMaxK * kExpandMaxK];
+  __shared__ int tok[kExpandMaxK * kExpandMaxK];
+  __shared__ uint64_t old_mask[2 * kExpandMaxK];
+  __shared__ int new_cs[kExpandMaxK];
   const int e = threadIdx.x;
   const int kk = k * k;
   const int base = k + level * kk;
@@ -93,14 +98,16 @@ __global__ void __launch_bounds__(1024) tree_expand_kernel(const float* __restri
     tb.front_src[e] = src;
     tb.front_ids[e] = tok[f];
     uint64_t m0 = old_mask[2 * src], m1 = old_mask[2 * src + 1];
-    if (col < 64) m0 |= 1ull << col; else m1 |= 1ull << (col - 64);
+    // the last level's own columns can lie beyond the two mask words (depth * k <= 128 bounds the columns a draft forward
+    // attends over, and nothing attends over the frontier the last level leaves): drop them rather than shift by >= 64
+    if (col < 64) m0 |= 1ull << col; else if (col < 128) m1 |= 1ull << (col - 64);
     tb.front_mask[2 * e] = m0;
     tb.front_mask[2 * e + 1] = m1;
   }
 }
 int launch_tree_expand(int dtype, const float* topk_p, const int* topk_i, const int64_t* d2t, int k, int level,
                        TreeBuffers tb, cudaStream_t s) {
-  if (k > 32) return static_cast<int>(cudaErrorInvalidValue);
+  if (k > kExpandMaxK) return static_cast<int>(cudaErrorInvalidValue);
   if (dtype == DT_BF16) launch_k(tree_expand_kernel<__nv_bfloat16>, dim3(1), dim3(1024), 0, s, 1, topk_p, topk_i, d2t, k, level, tb);
   else launch_k(tree_expand_kernel<__half>, dim3(1), dim3(1024), 0, s, 1, topk_p, topk_i, d2t, k, level, tb);
   return static_cast<int>(cudaGetLastError());
@@ -303,7 +310,13 @@ int launch_greedy_accept(const int* node_argmax, TreeBuffers tb, int T, int dept
 // KV compaction: utils.py:444-452.  Rows NPREV + sel[j] -> NPREV + j of every [kv_cap][128] plane.
 // Gather into registers first (the reference gathers into a temporary), then store: sources and destinations overlap.
 // --------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) kv_compact_kernel(uint4* kv, long plane_stride_v, long kv_cap, const int* sel, const int* st) {
+// One CTA moves at most kCompactRows rows (row j = threadIdx.x >> 4; rows beyond would be silently left in place).  A cycle
+// commits accept_length + 1 <= depth + 2 rows -- the root's token plus one per draft level, a whole retrieve row -- and
+// eb200_create keeps depth + 2 <= kMaxRetrieveWidth, so st[S_ACC] never reaches past the CTA's rows.  Raise both together.
+constexpr int kCompactRows = 16;
+constexpr int kMaxRetrieveWidth = 16;  // depth + 2 of the deepest accepted tree (eb200_create: depth <= 14)
+static_assert(kMaxRetrieveWidth <= kCompactRows, "kv_compact_kernel must cover a full-depth commit (depth + 2 rows)");
+__global__ void __launch_bounds__(kCompactRows * 16) kv_compact_kernel(uint4* kv, long plane_stride_v, long kv_cap, const int* sel, const int* st) {
   pdl_launch_dependents();
   pdl_wait();
   // sel / st are written by the accept kernel right before this one: dependent loads (see common.cuh:ld_dep)
@@ -320,7 +333,7 @@ __global__ void __launch_bounds__(256) kv_compact_kernel(uint4* kv, long plane_s
 int launch_kv_compact(int dtype, void* kv_base, long plane_stride, int n_planes, long kv_cap, const int* sel, const int* st,
                       cudaStream_t s) {
   (void)dtype;
-  launch_k(kv_compact_kernel, dim3(n_planes), dim3(256), 0, s, 1, reinterpret_cast<uint4*>(kv_base), plane_stride / 8, kv_cap, sel, st);
+  launch_k(kv_compact_kernel, dim3(n_planes), dim3(kCompactRows * 16), 0, s, 1, reinterpret_cast<uint4*>(kv_base), plane_stride / 8, kv_cap, sel, st);
   return static_cast<int>(cudaGetLastError());
 }
 

@@ -250,8 +250,18 @@ def draft_vocab_ids(vocab_size: int, draft_vocab_size: int) -> torch.Tensor:
 # named tiny fixtures shared by the golden generator (oracle/make_golden.py runs the unmodified reference on them),
 # the parity tests and bench.py's tp_parity check
 # --------------------------------------------------------------------------------------
+# a named fixture's weights under another draft-tree geometry: name -> (weights of, tree kwargs)
+GEOMETRY_FIXTURES = {
+    "e3_corr_bf16_D7": ("e3_corr_bf16", dict(total_token=60, depth=7, top_k=10)),      # EaModel.from_pretrained's default: 70 draft columns
+    "e3_corr_bf16_D8K16": ("e3_corr_bf16", dict(total_token=64, depth=8, top_k=16)),   # 128 draft columns, 64 verify rows
+}
+
+
 def fixture_models(name: str):
     """(tcfg, tW, hcfg, hW, eagle3, dtype, tree kwargs) for a named fixture; shared with tests."""
+    if name in GEOMETRY_FIXTURES:
+        base, tree = GEOMETRY_FIXTURES[name]
+        return fixture_models(base)[:6] + (dict(tree),)
     if name == "e3_rand_bf16":
         dtype, eagle3 = torch.bfloat16, True
         tcfg = target_config("tiny")
@@ -308,6 +318,8 @@ FIXTURES = {
     "e3_gqa_bf16": (70, 14, dict(temperature=0.0, max_new_tokens=40, max_length=512), None),
     "e1_rand_bf16": (21, 13, dict(temperature=0.0, max_new_tokens=16, max_length=512), None),
     "e3_tp8_bf16": (45, 15, dict(temperature=0.0, max_new_tokens=40, max_length=512), None),
+    "e3_corr_bf16_D7": (29, 11, dict(temperature=0.0, max_new_tokens=48, max_length=512), None),
+    "e3_corr_bf16_D8K16": (29, 11, dict(temperature=0.0, max_new_tokens=48, max_length=512), None),
     "e3_corr_bf16_T1": (29, 11, dict(temperature=1.0, max_new_tokens=32, max_length=512), 1234),
     # the HF warpers of utils.py:38-54 in action: temperature -> top-p -> top-k
     "e3_corr_bf16_T07": (29, 11, dict(temperature=0.7, top_p=0.9, top_k=20, max_new_tokens=32, max_length=512), 4321),

@@ -262,6 +262,16 @@ int eb200_k_tree_finalize(int32_t dtype, const float* scores, const int32_t* tok
                           int32_t depth, int32_t total_token, int32_t sample_token, int32_t sort_rows,
                           int64_t* draft_tokens, float* tree_mask, int64_t* tree_position_ids, int64_t* retrieve_indices,
                           int32_t* n_leaf, int32_t* max_depth);
+/* draft-tree growth (cnets.py:703-757) on host-supplied top-k tables: the level-0 seed, then one expansion per level.  HOST in/out.
+ * topk_p / topk_i [1 + depth*k][k]: row 0 = top-k of the stable pass' last row, rows 1 + l*k .. 1 + (l+1)*k = top-k of the k
+ * draft rows of level l (log-probs and draft-vocab ids); optional d2t [d2t_len]; last_row = the stable-pass row that seeds level 0.
+ * Outputs (any may be NULL): the candidate pool as eb200_k_tree_finalize takes it -- scores / tokens [k + depth*k*k],
+ * parents [1 + depth*k] -- and the frontier after the seed (slot 0) and after each level l (slot l + 1): front_ids / front_src /
+ * front_cs / front_scores [depth + 1][k], front_mask [depth + 1][k][2] (ancestor bits over draft tree columns, word 1 = columns
+ * 64..127).  k <= 32, depth <= 14, depth*k <= 128. */
+int eb200_k_tree_grow(int32_t dtype, const float* topk_p, const int32_t* topk_i, const int64_t* d2t, int32_t d2t_len, int32_t k,
+                      int32_t depth, int32_t last_row, float* scores, int32_t* tokens, int32_t* parents, int32_t* front_ids,
+                      int32_t* front_src, int32_t* front_cs, float* front_scores, uint64_t* front_mask);
 /* greedy posterior on a host-described tree (utils.py:360-373): node_argmax[T], draft_tokens[T],
  * retrieve[n_leaf*max_depth] -> best, accept_length, bonus token */
 int eb200_k_greedy_accept(const int32_t* node_argmax, const int32_t* draft_tokens, const int32_t* retrieve, int32_t T,

@@ -282,7 +282,7 @@ def make_static_goldens():
 
 # Fixtures whose float hidden-state captures (trees[*].in_hidden, cycles[*].hidden_new) no test reads: they are dropped so
 # that the stored file stays small (the tensor-parallel fixture is wide; with them it exceeds 1 MB).
-LEAN_FIXTURES = {"e3_tp8_bf16"}
+LEAN_FIXTURES = {"e3_tp8_bf16", "e3_corr_bf16_D7", "e3_corr_bf16_D8K16"}
 
 
 def main():
