@@ -102,6 +102,21 @@ static int make_tmap_w8(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t
                                      (unsigned long long)cols);
   return 0;
 }
+// W4A16 (launch_gemm_w4): the repacked nibble tiles [n_pad / 128][K / 64][4096 B] as rows of 256 B, box = one tile; the transposed
+// absmax [K / 64][n_pad] fp32, box = the 128 values of one tile
+static int make_tmap_w4(CUtensorMap* w, CUtensorMap* a, const void* tiles, const float* absmax, uint64_t n_pad, uint64_t K) {
+  TRY(resolve_encode());
+  const cuuint64_t wdims[2] = {256, n_pad * K / 2 / 256}, wstrides[1] = {256}, adims[2] = {n_pad, K / 64}, astrides[1] = {n_pad * 4};
+  const cuuint32_t wbox[2] = {256, 16}, abox[2] = {128, 1}, es[2] = {1, 1};
+  CUresult r = g_encode(w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(tiles), wdims, wstrides, wbox, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r == CUDA_SUCCESS)
+    r = g_encode(a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(absmax), adims, astrides, abox, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                 CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (4-bit) failed (%d) n_pad=%llu K=%llu", (int)r, (unsigned long long)n_pad,
+                                     (unsigned long long)K);
+  return 0;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // engine data
@@ -111,9 +126,12 @@ struct Linear {
   int N = 0, K = 0;
   int esize = 2;              // bytes per weight: 2 (model dtype) or 1 (int8, EB200_FLAG_TARGET_INT8)
   float* scale = nullptr;     // int8 only: fp32 scale of each row (SCB)
-  CUtensorMap tm;
+  float* absmax = nullptr;    // 4-bit only: w holds the repacked nibble tiles, absmax [K/64][n_pad] (launch_w4_repack)
+  int w4_quant = -1;          // 4-bit only: W4_NF4 / W4_FP4
+  int n_pad = 0;              // 4-bit only: N rounded up to whole 128-row tiles
+  CUtensorMap tm, tm_abs;     // tm_abs: 4-bit only
   uint64_t loaded_rows = 0;   // bookkeeping for fused / sharded loads
-  uint64_t loaded_scales = 0;
+  uint64_t loaded_scales = 0; // int8 SCB / 4-bit absmax
 };
 struct ActBuf {  // an activation buffer usable as the X operand of the GEMM (64 rows; 256 where the prompt prefill runs through it)
   void* p = nullptr;
@@ -276,9 +294,19 @@ static int dalloc(eb200_engine* e, void** p, size_t bytes, bool zero = true) {
   if (zero) CK(cudaMemsetAsync(*p, 0, bytes, e->stream));
   return 0;
 }
-static int alloc_linear(eb200_engine* e, Linear& l, int N, int K, bool int8 = false) {
+// wq: 0 model dtype, EB200_FLAG_TARGET_INT8 / _NF4 / _FP4
+static int alloc_linear(eb200_engine* e, Linear& l, int N, int K, int wq = 0) {
   l.N = N;
   l.K = K;
+  if (wq == EB200_FLAG_TARGET_NF4 || wq == EB200_FLAG_TARGET_FP4) {
+    if (K % 64) return fail("4-bit target weights need in-features divisible by 64 (blocksize 64 blocks must not straddle rows), got %d", K);
+    l.w4_quant = wq == EB200_FLAG_TARGET_NF4 ? W4_NF4 : W4_FP4;
+    l.n_pad = (N + 127) / 128 * 128;
+    l.esize = 1;  // per two weights
+    TRY(dalloc(e, reinterpret_cast<void**>(&l.absmax), static_cast<size_t>(l.n_pad) * (K / 64) * 4));
+    return dalloc(e, &l.w, static_cast<size_t>(l.n_pad) * K / 2);
+  }
+  const bool int8 = wq == EB200_FLAG_TARGET_INT8;
   l.esize = int8 ? 1 : 2;
   if (int8) TRY(dalloc(e, reinterpret_cast<void**>(&l.scale), static_cast<size_t>(N) * 4, false));
   return dalloc(e, &l.w, static_cast<size_t>(N) * K * l.esize, false);
@@ -316,6 +344,14 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
   if (c.tp_size < 1 || c.tp_rank < 0 || c.tp_rank >= c.tp_size) return fail("bad tp rank/size");
   if (c.num_heads % c.tp_size || c.num_kv_heads % c.tp_size || c.intermediate_size % c.tp_size)
     return fail("heads / kv heads / intermediate size must divide by tp_size");
+  {
+    const int wq = c.flags & (EB200_FLAG_TARGET_INT8 | EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4);
+    if (wq & (wq - 1)) return fail("EB200_FLAG_TARGET_INT8, EB200_FLAG_TARGET_NF4 and EB200_FLAG_TARGET_FP4 exclude each other");
+    // the 4-bit loader places whole checkpoint tensors (no tensor-parallel sharding of codes or absmax)
+    if ((wq & (EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4)) && c.tp_size > 1)
+      return fail("4-bit target weights (EB200_FLAG_TARGET_NF4 / _FP4) are not supported with tensor parallelism (tp_size %d); "
+                  "they run on one GPU", c.tp_size);
+  }
   if (c.total_token < 2 || c.total_token > 64) return fail("total_token must be in [2, 64]");
   if (c.top_k < 1 || c.top_k > 16) return fail("top_k must be in [1, 16]");
   if (c.depth < 1 || c.depth + 2 > 16) return fail("depth must be in [1, 14]");
@@ -383,12 +419,12 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
     // ---- target weights
     TRY(dalloc(e, &e->t_embed, static_cast<size_t>(e->V) * H * 2, false));
     e->tl.resize(e->L);
-    const bool w8 = (c.flags & EB200_FLAG_TARGET_INT8) != 0;
+    const int wq = c.flags & (EB200_FLAG_TARGET_INT8 | EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4);
     for (auto& l : e->tl) {
-      TRY(alloc_linear(e, l.qkv, (e->nh_l + 2 * e->nkv_l) * 128, H, w8));
-      TRY(alloc_linear(e, l.o, H, e->nh_l * 128, w8));
-      TRY(alloc_linear(e, l.gu, 2 * e->I_l, H, w8));
-      TRY(alloc_linear(e, l.down, H, e->I_l, w8));
+      TRY(alloc_linear(e, l.qkv, (e->nh_l + 2 * e->nkv_l) * 128, H, wq));
+      TRY(alloc_linear(e, l.o, H, e->nh_l * 128, wq));
+      TRY(alloc_linear(e, l.gu, 2 * e->I_l, H, wq));
+      TRY(alloc_linear(e, l.down, H, e->I_l, wq));
       TRY(dalloc(e, &l.ln1, H * 2, false));
       TRY(dalloc(e, &l.ln2, H * 2, false));
     }
@@ -654,26 +690,47 @@ static bool ends_with(const std::string& s, const char* suf) {
   const size_t n = strlen(suf);
   return s.size() >= n && s.compare(s.size() - n, n, suf) == 0;
 }
-// the seven decoder-layer projections: weight "<proj>.weight"; int8 row scales "<proj>.SCB" (EB200_FLAG_TARGET_INT8)
+// the seven decoder-layer projections: weight "<proj>.weight"; int8 row scales "<proj>.SCB" (EB200_FLAG_TARGET_INT8); 4-bit block
+// absmax "<proj>.weight.absmax" (EB200_FLAG_TARGET_NF4 / _FP4)
 static const char* const kProjNames[7] = {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj",
                                           "mlp.gate_proj",    "mlp.up_proj",      "mlp.down_proj"};
-static int proj_index(const std::string& sub, bool* scb) {
+enum ProjPart { PART_WEIGHT = 0, PART_SCB = 1, PART_ABSMAX = 2 };
+static int proj_index(const std::string& sub, int* part) {
   for (int i = 0; i < 7; ++i) {
     const std::string p(kProjNames[i]);
-    if (sub == p + ".weight" || sub == p + ".SCB") {
-      *scb = sub == p + ".SCB";
+    if (sub == p + ".weight" || sub == p + ".SCB" || sub == p + ".weight.absmax") {
+      *part = sub == p + ".weight" ? PART_WEIGHT : sub == p + ".SCB" ? PART_SCB : PART_ABSMAX;
       return i;
     }
   }
   return -1;
+}
+// 4-bit: copy the [nr][C] tensor (nibbles, or absmax with C = K / 64) to the device and repack its rows into the engine's layout
+static int load_w4(eb200_engine* e, Linear& L, bool absmax, const void* data, long nr, long row0, int half) {
+  const long rows_needed = half >= 0 ? nr * 2 : row0 + nr;  // gate/up: the two halves interleave over 2 * nr rows
+  if (nr < 0 || row0 < 0 || (half >= 0 && nr % 64) || rows_needed > L.N)
+    return fail("4-bit load: %ld source rows at destination row %ld do not fit the %d rows of the projection", nr, row0, L.N);
+  const size_t bytes = absmax ? static_cast<size_t>(nr) * (L.K / 64) * 4 : static_cast<size_t>(nr) * L.K / 2;
+  void* tmp = nullptr;
+  CK(cudaMalloc(&tmp, bytes));
+  int rc = 0;
+  if (cudaMemcpyAsync(tmp, data, bytes, cudaMemcpyDefault, e->stream) != cudaSuccess) rc = fail("4-bit load: copy failed");
+  else if (launch_w4_repack(absmax ? nullptr : static_cast<const uint8_t*>(tmp), absmax ? static_cast<const float*>(tmp) : nullptr,
+                            static_cast<int>(nr), L.K, static_cast<int>(row0), half, static_cast<uint8_t*>(L.w), L.absmax, L.n_pad,
+                            e->stream) != 0 ||
+           cudaStreamSynchronize(e->stream) != cudaSuccess)
+    rc = fail("4-bit load: repack failed");
+  cudaFree(tmp);
+  return rc;
 }
 
 static int load_layer_tensor(eb200_engine* e, Layer& l, const std::string& sub, const void* data, const int64_t* shape,
                              int nd, bool is_target, int Hin_qkv, int Hm, int nh_full, int nkv_full, int I_full) {
   const int tp = is_target ? e->c.tp_size : 1, rk = is_target ? e->c.tp_rank : 0;
   const int nh_l = nh_full / tp, nkv_l = nkv_full / tp;
-  bool scb = false;
-  const int pi = proj_index(sub, &scb);
+  int part = PART_WEIGHT;
+  const int pi = proj_index(sub, &part);
+  const bool scb = part == PART_SCB;
   if (pi >= 0) {
     // destination matrix, full [rows, cols] of the checkpoint tensor, first destination row, gate/up half, loaded bit
     struct Slot {
@@ -693,7 +750,17 @@ static int load_layer_tensor(eb200_engine* e, Layer& l, const std::string& sub, 
     const std::string wname = std::string(kProjNames[pi]) + ".weight";
     const Shard sh = shard_of(wname, sl.rows, sl.cols, rk, tp);
     Linear& L = *sl.lin;
-    if (!scb) {
+    if (L.absmax) {  // 4-bit (one GPU: the shard is the whole tensor)
+      if (part == PART_SCB) return fail("%s.SCB: row scales belong to int8 projections; this engine stores 4-bit weights", short_name);
+      const bool am = part == PART_ABSMAX;
+      if (!shape_is(shape, nd, sl.rows, am ? sl.cols / 64 : sl.cols / 2))
+        return fail("%s%s shape mismatch (want [%ld, %ld] %s)", short_name, am ? ".weight.absmax" : ".weight", sl.rows,
+                    am ? sl.cols / 64 : sl.cols / 2, am ? "fp32" : "uint8: two 4-bit codes per byte");
+      TRY(load_w4(e, L, am, data, sl.rows, sl.row0, sl.half));
+      (am ? L.loaded_scales : L.loaded_rows) |= sl.bit;
+    } else if (part == PART_ABSMAX) {
+      return fail("%s.weight.absmax: block absmax belongs to 4-bit projections (EB200_FLAG_TARGET_NF4 / _FP4)", short_name);
+    } else if (!scb) {
       if (!shape_is(shape, nd, sl.rows, sl.cols)) return fail("%s shape mismatch", short_name);
       if (sl.half >= 0) TRY(copy_interleaved64(e, L.w, sl.half, data, sl.cols, sh, L.esize));
       else TRY(copy_block(e, L.w, sl.row0, data, sl.cols, sh.r0, sh.nr, sh.c0, sh.nc, L.esize));
@@ -733,11 +800,27 @@ extern "C" int eb200_load_tensor(eb200_engine* e, const char* name_c, const void
   const bool want_model_dtype = !(name == "head.d2t" || name == "head.t2d");
   const eb200_config& c = e->c;
   // int8 target projections: "<proj>.weight" int8 + "<proj>.SCB" fp32, only on an engine created with EB200_FLAG_TARGET_INT8
-  bool scb = false;
+  int part = PART_WEIGHT;
   const bool target_proj = !is_head && name.rfind("model.layers.", 0) == 0 && name.find('.', strlen("model.layers.")) != std::string::npos &&
-                           proj_index(name.substr(name.find('.', strlen("model.layers.")) + 1), &scb) >= 0;
+                           proj_index(name.substr(name.find('.', strlen("model.layers.")) + 1), &part) >= 0;
+  const bool scb = part == PART_SCB;
   const bool w8 = (c.flags & EB200_FLAG_TARGET_INT8) != 0;
-  if (dtype == EB200_DT_INT8 || ends_with(name, ".SCB")) {
+  const bool w4 = (c.flags & (EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4)) != 0;
+  if (dtype == EB200_DT_UINT8 || ends_with(name, ".absmax")) {
+    // 4-bit target projections: "<proj>.weight" uint8 + "<proj>.weight.absmax" fp32
+    if (!target_proj)
+      return fail("tensor '%s': 4-bit codes and absmax are accepted only for the target decoder projections (q/k/v/o/gate/up/down_proj); "
+                  "embeddings, norms, lm_head and the draft head stay in the model dtype", name_c);
+    if (!w4) return fail("tensor '%s': 4-bit data for an engine created without EB200_FLAG_TARGET_NF4 / _FP4 (load_in_4bit)", name_c);
+    if (part == PART_ABSMAX && dtype != EB200_DT_FP32) return fail("tensor '%s': 4-bit block absmax must be fp32", name_c);
+    if (part == PART_WEIGHT && dtype != EB200_DT_UINT8) return fail("tensor '%s': 4-bit weights must be uint8 (two codes per byte)", name_c);
+  } else if (w4 && target_proj && (dtype == EB200_DT_INT8 || scb)) {
+    return fail("tensor '%s': int8 data (load_in_8bit format) for an engine that stores the target projections in 4 bits "
+                "(EB200_FLAG_TARGET_NF4 / _FP4)", name_c);
+  } else if (w4 && target_proj) {
+    return fail("tensor '%s': this engine stores the target projections in 4 bits (EB200_FLAG_TARGET_NF4 / _FP4): pass the uint8 codes and "
+                "their fp32 block absmax (eagle_b200.quant.quantize_4bit)", name_c);
+  } else if (dtype == EB200_DT_INT8 || ends_with(name, ".SCB")) {
     if (!target_proj)
       return fail("tensor '%s': int8 weights and SCB row scales are accepted only for the target decoder projections "
                   "(q/k/v/o/gate/up/down_proj); embeddings, norms, lm_head and the draft head stay in the model dtype", name_c);
@@ -848,6 +931,10 @@ extern "C" int eb200_set_rope_table(eb200_engine* e, int32_t which, const void* 
 
 static int finalize_linear(eb200_engine* e, Linear& l, const char* what, uint64_t need) {
   if (l.loaded_rows != need) return fail("weights missing for %s", what);
+  if (l.absmax) {
+    if (l.loaded_scales != need) return fail("block absmax missing for %s (4-bit weights need their fp32 .weight.absmax)", what);
+    return make_tmap_w4(&l.tm, &l.tm_abs, l.w, l.absmax, l.n_pad, l.K);
+  }
   if (l.scale) {
     if (l.loaded_scales != need) return fail("SCB row scales missing for %s (int8 weights need their fp32 row scales)", what);
     return make_tmap_w8(&l.tm, l.w, l.N, l.K);
@@ -859,8 +946,10 @@ static int gemm_mode();
 extern "C" int eb200_finalize(eb200_engine* e) {
   if (!e) return fail("eb200_finalize: null engine");
   CK(cudaSetDevice(e->c.device));
-  if (e->c.flags & EB200_FLAG_TARGET_INT8) {
-    // the W8A16 GEMM exists as the cluster split-K kernel of one GPU only
+  if (e->c.flags & (EB200_FLAG_TARGET_INT8 | EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4)) {
+    // the W8A16 / W4A16 GEMMs exist as the cluster split-K kernel of one GPU only
+    const char* fmt = (e->c.flags & EB200_FLAG_TARGET_INT8) ? "int8 target weights (EB200_FLAG_TARGET_INT8)"
+                                                             : "4-bit target weights (EB200_FLAG_TARGET_NF4 / _FP4)";
     const char* what = nullptr;
     const char* chain = getenv("EB200_CHAIN");
     if (e->c.tp_size > 1) what = "tensor parallelism (tp_size > 1)";
@@ -868,8 +957,7 @@ extern "C" int eb200_finalize(eb200_engine* e) {
     else if (chain && atoi(chain) == 1) what = "EB200_CHAIN=1 (persistent layer-segment launches)";
     else if (gemm_mode() == 0) what = "EB200_GEMM_MODE=streamk";
     if (what)
-      return fail("int8 target weights (EB200_FLAG_TARGET_INT8) are not supported with %s; they run on one GPU with the default "
-                  "cluster split-K GEMM", what);
+      return fail("%s are not supported with %s; they run on one GPU with the default cluster split-K GEMM", fmt, what);
   }
   char nm[128];
   if (!e->t_embed_loaded || !e->t_norm_loaded) return fail("target embed/norm weights missing");
@@ -1074,7 +1162,8 @@ static L2Prefetch l2_plan(const eb200_engine* e, const Linear& next, int mpad, i
   L2Prefetch pf;
   memset(&pf, 0, sizeof(pf));
   pf.j0 = pf.j1 = j0;
-  if (!l2_prefetch_on() || !next.w || next.N <= 0 || next.K <= 0 || bytes <= 0) return pf;
+  // 4-bit weights are not prefetched: their tiles and absmax are two maps with other boxes than the plan's
+  if (!l2_prefetch_on() || !next.w || next.absmax || next.N <= 0 || next.K <= 0 || bytes <= 0) return pf;
   pf.tm = next.tm;
   pf.n_tiles = (next.N + 127) / 128;
   pf.splitk = pick_splitk(next.N, next.K, mpad, 0, e->ws_bytes);
@@ -1112,8 +1201,10 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
   p.splitk = pick_splitk(p.N, p.K, cx.mpad, g.epi, e->ws_bytes);
   if ((p.N + 127) / 128 > 8192) return fail("too many n tiles");
   p.w_scale = g.W->scale;
-  // algorithmic weight bytes: int8 weights stream N*K bytes plus the N fp32 row scales
-  const double bytes = p.w_scale ? static_cast<double>(p.N) * p.K + 4.0 * p.N : static_cast<double>(p.N) * p.K * 2 * (g.epi == EPI_SWIGLU ? 2 : 1);
+  p.w4_quant = g.W->w4_quant;
+  // algorithmic weight bytes: int8 weights stream N*K bytes plus the N fp32 row scales; 4-bit ones N*K/2 plus N*K/64 fp32 absmax
+  const double nk = static_cast<double>(p.N) * p.K;
+  const double bytes = g.W->absmax ? nk / 2 + 4.0 * nk / 64 : p.w_scale ? nk + 4.0 * p.N : nk * 2 * (g.epi == EPI_SWIGLU ? 2 : 1);
   const char* kname = g.epi == EPI_STORE ? "gemm_store" : g.epi == EPI_RESIDUAL ? "gemm_residual" :
                       (g.epi == EPI_SWIGLU || g.epi == EPI_SWIGLU_IL) ? "gemm_swiglu" : "gemm_qkv_rope";
   {
@@ -1122,7 +1213,11 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
     if (skip_kernel(kname) || skip_kernel(kk)) return 0;
   }
   ProfScope ps(e, 0, bytes, kname);
-  if (p.w_scale) {
+  if (g.W->absmax) {
+    if (cx.mpad == 256 && g.X->rows < 256) return fail("256-row GEMM on a 64-row activation buffer");
+    CKL(launch_gemm_w4(e->dtype, cx.mpad, g.epi, &g.W->tm, &g.W->tm_abs, cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256),
+                       p, e->stream, g.pf));
+  } else if (p.w_scale) {
     if (cx.mpad == 256 && g.X->rows < 256) return fail("256-row GEMM on a 64-row activation buffer");
     CKL(launch_gemm_w8(e->dtype, cx.mpad, g.epi, &g.W->tm, cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256), p,
                        e->stream, g.pf));
@@ -2799,6 +2894,53 @@ extern "C" int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, 
   CKL(launch_gemm_w8(dtype, mpad, epilogue, &tw, &tx, p, s));
   CK(cudaStreamSynchronize(s));
   return 0;
+}
+
+extern "C" int eb200_k_gemm_w4(int32_t dtype, int32_t quant_type, int32_t epilogue, const void* Wq, const void* absmax, const void* X, void* out,
+                               const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream) {
+  if (M < 1 || M > 64 || (epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !absmax || splitk < 1 ||
+      splitk > 8 || N < 1 || K < 64 || K % 64 || (quant_type != W4_NF4 && quant_type != W4_FP4))
+    return fail("eb200_k_gemm_w4: bad arguments");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const int mpad = M <= 16 ? 16 : 64;
+  const int n_out = N;  // EPI_SWIGLU_IL: Wq is the [2N, K/2] interleaved gate/up matrix, out is [M, N]
+  if (epilogue == EPI_SWIGLU_IL) {
+    if (N % 64) return fail("eb200_k_gemm_w4: interleaved SwiGLU needs N % 64 == 0");
+    N *= 2;
+  }
+  GemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.N = N;
+  p.K = K;
+  p.m_rows = M;
+  p.m_idx = -1;
+  p.splitk = splitk;
+  p.out = out;
+  p.ld_out = n_out;
+  p.res = res;
+  p.ld_res = n_out;
+  p.bias = bias;
+  p.w4_quant = quant_type;
+  const int n_pad = (N + 127) / 128 * 128;
+  const size_t tile_bytes = static_cast<size_t>(n_pad) * K / 2, abs_bytes = static_cast<size_t>(n_pad) * (K / 64) * 4;
+  void* buf = nullptr;
+  CK(cudaMalloc(&buf, tile_bytes + abs_bytes));
+  uint8_t* tiles = static_cast<uint8_t*>(buf);
+  float* am = reinterpret_cast<float*>(tiles + tile_bytes);
+  int rc = 0;
+  CUtensorMap tw, ta, tx;
+  if (cudaMemsetAsync(buf, 0, tile_bytes + abs_bytes, s) != cudaSuccess ||
+      launch_w4_repack(static_cast<const uint8_t*>(Wq), static_cast<const float*>(absmax), N, K, 0, -1, tiles, am, n_pad, s) != 0)
+    rc = fail("eb200_k_gemm_w4: repack failed");
+  if (!rc) rc = make_tmap_w4(&tw, &ta, tiles, am, n_pad, K);
+  if (!rc) rc = make_tmap(&tx, dtype, X, 64, K, mpad);
+  if (!rc) {
+    const int r = launch_gemm_w4(dtype, mpad, epilogue, &tw, &ta, &tx, p, s);
+    if (r != 0) rc = fail("eb200_k_gemm_w4: launch failed (%d)", r);
+  }
+  if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = fail("eb200_k_gemm_w4: %s", cudaGetErrorString(cudaGetLastError()));
+  cudaFree(buf);
+  return rc;
 }
 
 // One decoder-layer segment through the persistent chain kernel (mega.cu), on caller tensors (all DEVICE pointers):

@@ -22,6 +22,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+
 #include "gemm_common.cuh"
 
 namespace eb {
@@ -45,10 +47,12 @@ static int smem_budget(int total_ctas) {
   }
   return (total_ctas <= device_sm_count() ? big_kb : small_kb) * 1024;
 }
-static int stage_count_for(int mpad, int epi, int total_ctas, bool w8 = false) {
+static int stage_count_for(int mpad, int epi, int total_ctas, int wq = WQ_NONE) {
   // 256 activation rows (prefill): a stage is 48 KB and the cluster reduction parks 128 KB of partials, so always one CTA per SM
   const int budget = mpad >= 256 ? 200 * 1024 : smem_budget(total_ctas);
-  int s = w8 ? (budget - kCtrlBytes - 1024 - kW8DqBytes) / stage_bytes_w8(mpad) : (budget - kCtrlBytes - 1024) / stage_bytes(mpad, epi);
+  int s = wq == WQ_INT8   ? (budget - kCtrlBytes - 1024 - kW8DqBytes) / stage_bytes_w8(mpad)
+          : wq == WQ_4BIT ? (budget - kCtrlBytes - 1024) / stage_bytes_w4(mpad)
+                          : (budget - kCtrlBytes - 1024) / stage_bytes(mpad, epi);
   if (s > kMaxStages) s = kMaxStages;
   if (s < 2) s = 2;
   return s;
@@ -101,6 +105,30 @@ template <typename T> __device__ __forceinline__ void dequant_w8_rows(uint32_t s
                  : "memory");
   }
 }
+// W4A16: bitsandbytes' code tables (quant.py NF4_CODE / FP4_CODE, the constants of its dDequantizeNF4 / dDequantizeFP4Tree).  In global
+// memory rather than a __constant__ bank: with a user constant bank in this module every GEMM launch of a replayed cycle graph measured
+// slower on the H100, the model-dtype ones included.
+__device__ const float kW4Codes[2][16] = {
+    {-1.0f, -0.6961928009986877f, -0.5250730514526367f, -0.39491748809814453f, -0.28444138169288635f, -0.18477343022823334f,
+     -0.09105003625154495f, 0.0f, 0.07958029955625534f, 0.16093020141458511f, 0.24611230194568634f, 0.33791524171829224f,
+     0.44070982933044434f, 0.5626170039176941f, 0.7229568362236023f, 1.0f},
+    {0.0f, 0.0052083333f, 0.66666667f, 1.0f, 0.33333333f, 0.5f, 0.16666667f, 0.25f, -0.0f, -0.0052083333f, -0.66666667f, -1.0f,
+     -0.33333333f, -0.5f, -0.16666667f, -0.25f}};
+// One k16 step of a thread's A fragment from its 4 repacked bytes w (byte i -> register i; the high nibble is the lower K column):
+// T(code * absmax) with one __fmul_rn; s0 / s1 are the absmax of its rows r0 / r0 + 8 (registers 0, 2 / 1, 3).  The 16-entry table
+// lives in shared memory: its entries fall in 16 distinct banks, so the lookups are conflict-free.
+template <typename T>
+__device__ __forceinline__ void w4_fragment(uint32_t w, uint32_t lut, float s0, float s1, uint32_t (&a)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float lo, hi;
+    asm("ld.shared.f32 %0, [%1];" : "=f"(lo) : "r"(lut + ((w >> (8 * i + 2)) & 0x3Cu)));
+    asm("ld.shared.f32 %0, [%1];" : "=f"(hi) : "r"(lut + ((w << 2 >> (8 * i)) & 0x3Cu)));
+    const float sc = (i & 1) ? s1 : s0;
+    a[i] = pack2_rn<T>(__fmul_rn(lo, sc), __fmul_rn(hi, sc));
+  }
+}
+
 __device__ __forceinline__ float ld_global_f32(const float* p) {
   float v;
   asm volatile("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
@@ -121,16 +149,22 @@ __device__ __forceinline__ float ld_global_f32(const float* p) {
 // warpgroup) and run the same k16 MMAs on it, so the accumulators equal those of the kernel on the dequantized W.  Each k-block's
 // MMAs retire before the next dequantization (wgmma_wait<0>): ptxas serialises every wgmma of a kernel whose MMAs stay in flight
 // across the conversion code.  The other warpgroup and the second resident CTA keep the tensor pipe and the TMA ring busy meanwhile.
-template <typename T, int MPAD, int EPI, bool XMC, bool W8>
+// W4: tmW streams 4 KB nibble tiles in fragment order and tmW2 (unused by the single-matrix epilogues W4 serves) the tile's absmax.
+// Each thread reads its 16 nibble bytes of a k-block with one shared load and converts one k16 step at a time straight into the A
+// registers of a wgmma RS: step k + 1 is converted while step k's MMA runs (two fragment buffers, one commit group per step,
+// wgmma_wait<1>), so neither a shared-memory round trip nor a proxy fence sits on the MMA chain.
+template <typename T, int MPAD, int EPI, bool XMC, int WQ>
 __global__ void __launch_bounds__(kGemmThreads, (MPAD >= 256 ? 1 : 2))
 skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmW2,
                   const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXh, const GemmParams p, const int stages,
                   const __grid_constant__ L2Prefetch pf) {
   constexpr bool kDual = (EPI == EPI_SWIGLU);
+  constexpr bool W8 = WQ == WQ_INT8, W4 = WQ == WQ_4BIT;
   static_assert(!XMC || (MPAD == 64 && !kDual), "X multicast: 64-row tiles, single accumulator");
-  static_assert(!W8 || (!XMC && !kDual), "W8A16: single weight stream, no X multicast");
-  constexpr int kWBytes = W8 ? kW8TileBytes : kWTileBytes;  // weight bytes of one stage (per weight matrix)
-  constexpr int kStageBytes = W8 ? stage_bytes_w8(MPAD) : stage_bytes(MPAD, EPI);
+  static_assert(WQ == WQ_NONE || (!XMC && !kDual), "W8A16 / W4A16: single weight stream, no X multicast");
+  constexpr int kWBytes = W8 ? kW8TileBytes : W4 ? kW4WBytes : kWTileBytes;  // weight bytes of one stage (per weight matrix)
+  constexpr int kStageBytes = W8 ? stage_bytes_w8(MPAD) : W4 ? stage_bytes_w4(MPAD) : stage_bytes(MPAD, EPI);
+  constexpr int kTxBytes = W4 ? kW4TileBytes + kW4AbsBytes + x_tile_bytes(MPAD) : kStageBytes;  // bytes TMA lands per stage
   constexpr int kPartBytes = acc_tile_bytes(MPAD, EPI);
 
   extern __shared__ uint8_t smem_raw[];
@@ -139,6 +173,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
   uint8_t* ctrl = wdq + (W8 ? kW8DqBytes : 0);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);
   uint64_t* empty_bar = full_bar + kMaxStages;
+  float* w4_lut = reinterpret_cast<float*>(ctrl + 512);  // W4: the code table
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -175,12 +210,18 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
       // (written by the predecessor) follow after the wait; both land on the same full barrier (tx bytes add up).
       const int nkb = kb_end - kb_begin;
       const int pre = nkb < stages ? nkb : stages;
-      for (int j = 0; j < pre; ++j) {
-        uint8_t* st = smem + j * kStageBytes;
-        mbar_arrive_expect_tx(&full_bar[j], kStageBytes);
-        tma_load_2d(st, &tmW, &full_bar[j], (kb_begin + j) * kBlockK, n_tile * kBlockN, kEvictFirst);
-        if (kDual) tma_load_2d(st + kWTileBytes, &tmW2, &full_bar[j], (kb_begin + j) * kBlockK, n_tile * kBlockN, kEvictFirst);
-      }
+      auto load_w = [&](int stage, int kb) {
+        uint8_t* st = smem + stage * kStageBytes;
+        mbar_arrive_expect_tx(&full_bar[stage], kTxBytes);
+        if constexpr (W4) {
+          tma_load_2d(st, &tmW, &full_bar[stage], 0, (n_tile * num_kb + kb) * (kW4TileBytes / 256), kEvictFirst);
+          tma_load_2d(st + kW4TileBytes, &tmW2, &full_bar[stage], n_tile * kBlockN, kb, kEvictFirst);
+        } else {
+          tma_load_2d(st, &tmW, &full_bar[stage], kb * kBlockK, n_tile * kBlockN, kEvictFirst);
+          if (kDual) tma_load_2d(st + kWTileBytes, &tmW2, &full_bar[stage], kb * kBlockK, n_tile * kBlockN, kEvictFirst);
+        }
+      };
+      for (int j = 0; j < pre; ++j) load_w(j, kb_begin + j);
       pdl_wait();
       auto load_x = [&](int stage, int kb) {
         uint8_t* xdst = smem + stage * kStageBytes + kWBytes * (kDual ? 2 : 1);
@@ -196,10 +237,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
       uint32_t ph = (pre == stages) ? 1 : 0;
       for (int kb = kb_begin + pre; kb < kb_end; ++kb) {
         mbar_wait_mma(&empty_bar[s], ph ^ 1);
-        uint8_t* st = smem + s * kStageBytes;
-        mbar_arrive_expect_tx(&full_bar[s], kStageBytes);
-        tma_load_2d(st, &tmW, &full_bar[s], kb * kBlockK, n_tile * kBlockN, kEvictFirst);
-        if (kDual) tma_load_2d(st + kWTileBytes, &tmW2, &full_bar[s], kb * kBlockK, n_tile * kBlockN, kEvictFirst);
+        load_w(s, kb);
         load_x(s, kb);
         if (++s == stages) {
           s = 0;
@@ -236,7 +274,56 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     }
     int s = 0, prev = -1;
     uint32_t ph = 0;
-    for (int kb = kb_begin; kb < kb_end; ++kb) {
+    if constexpr (W4) {
+      pdl_wait();  // the code table is read with a generic load, which may not precede the dependency wait (X tiles follow it anyway)
+      if (threadIdx.x < 16)
+        asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_u32(w4_lut + threadIdx.x)), "f"(ld_global_f32(&kW4Codes[p.w4_quant][threadIdx.x]))
+                     : "memory");
+      asm volatile("bar.sync 2, 256;" ::: "memory");  // both MMA warpgroups see the table
+      // thread t of the warpgroup: its 16 bytes of every tile at (wg * 128 + t) * 16, word k = k16 step k; absmax of rows r0, r0 + 8
+      const uint32_t lut = smem_u32(w4_lut);
+      const int t = threadIdx.x & 127;
+      const int r0 = wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+      uint32_t q[4], a[2][4];
+      float s0 = 0.f, s1 = 0.f;
+      auto fetch = [&](int stage) {
+        const uint32_t st = smem_u32(smem + stage * kStageBytes);
+        asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]) : "r"(st + (threadIdx.x & 255) * 16)
+                     : "memory");
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(s0) : "r"(st + kW4TileBytes + r0 * 4) : "memory");
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(s1) : "r"(st + kW4TileBytes + (r0 + 8) * 4) : "memory");
+      };
+      if (kb_begin < kb_end) {
+        mbar_wait_mma(&full_bar[0], 0);
+        fetch(0);
+        w4_fragment<T>(q[0], lut, s0, s1, a[0]);
+      }
+      for (int kb = kb_begin; kb < kb_end; ++kb) {
+        const uint64_t b_desc = make_kmajor_sw128_desc(smem_u32(smem + s * kStageBytes) + kWBytes);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_fence();
+          WgmmaRS<T, MPAD>::mma(acc, a[k & 1], b_desc + 2 * k);
+          wgmma_commit();
+          wgmma_wait<1>();  // step k - 1 has retired: its fragment buffer a[(k + 1) & 1] may be rewritten
+          if (k == 0 && prev >= 0) release(prev);  // ... and with it the previous k-block's last MMA
+          if (k < 3) {
+            w4_fragment<T>(q[k + 1], lut, s0, s1, a[(k + 1) & 1]);
+          } else if (kb + 1 < kb_end) {
+            const int sn = s + 1 == stages ? 0 : s + 1;
+            mbar_wait_mma(&full_bar[sn], sn == 0 ? ph ^ 1 : ph);
+            fetch(sn);
+            w4_fragment<T>(q[0], lut, s0, s1, a[0]);
+          }
+        }
+        prev = s;
+        if (++s == stages) {
+          s = 0;
+          ph ^= 1;
+        }
+      }
+    }
+    for (int kb = kb_begin; kb < kb_end && !W4; ++kb) {
       mbar_wait_mma(&full_bar[s], ph);
       const uint32_t st = smem_u32(smem + s * kStageBytes);
       uint32_t a_addr = st + wg * (kWTileBytes / 2);  // 64 weight rows = 8 KB = eight whole swizzle atoms
@@ -428,7 +515,7 @@ static bool xmc_enabled() {
   }
   return v == 1;
 }
-template <typename T, int MPAD, int EPI, bool XMC, bool W8 = false>
+template <typename T, int MPAD, int EPI, bool XMC, int WQ = WQ_NONE>
 static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
                         cudaStream_t s, const L2Prefetch* pf);
 template <typename T, int MPAD, int EPI>
@@ -440,14 +527,14 @@ static int launch_one(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUt
   }
   return launch_one_x<T, MPAD, EPI, false>(tmW, tmW2, tmX, tmX, p, s, pf);
 }
-template <typename T, int MPAD, int EPI, bool XMC, bool W8>
+template <typename T, int MPAD, int EPI, bool XMC, int WQ>
 static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
                         cudaStream_t s, const L2Prefetch* pf) {
-  auto kern = skinny_gemm_wgmma<T, MPAD, EPI, XMC, W8>;
+  auto kern = skinny_gemm_wgmma<T, MPAD, EPI, XMC, WQ>;
   dim3 grid((p.N + kBlockN - 1) / kBlockN, p.splitk);
-  const int stages = stage_count_for(MPAD, EPI, static_cast<int>(grid.x * grid.y), W8);
-  const int sbytes = W8 ? stage_bytes_w8(MPAD) : stage_bytes(MPAD, EPI);
-  const int smem = stages * sbytes + (W8 ? kW8DqBytes : 0) + kCtrlBytes + 1024;
+  const int stages = stage_count_for(MPAD, EPI, static_cast<int>(grid.x * grid.y), WQ);
+  const int sbytes = WQ == WQ_INT8 ? stage_bytes_w8(MPAD) : WQ == WQ_4BIT ? stage_bytes_w4(MPAD) : stage_bytes(MPAD, EPI);
+  const int smem = stages * sbytes + (WQ == WQ_INT8 ? kW8DqBytes : 0) + kCtrlBytes + 1024;
   if (p.splitk > 8) return static_cast<int>(cudaErrorInvalidValue);  // portable cluster size
   // the accumulators are parked as (1|2) x MPAD x 128 fp32 partials (+ a 4 KB exchange strip) in the stage memory
   if (stages * sbytes < acc_tile_bytes(MPAD, EPI) + 4096)
@@ -512,16 +599,35 @@ int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUte
   return static_cast<int>(cudaErrorInvalidValue);
 }
 
-// W8A16: the epilogues of the target's decoder layer (+ EPI_STORE for mpad 16 / 64)
-template <typename T, int MPAD>
-static int launch_w8_epi(int epi, const CUtensorMap* w, const CUtensorMap* x, const GemmParams& p, cudaStream_t s, const L2Prefetch* pf) {
+// W8A16 / W4A16: the epilogues of the target's decoder layer (+ EPI_STORE for mpad 16 / 64); w2: W4's absmax map
+template <typename T, int MPAD, int WQ>
+static int launch_wq_epi(int epi, const CUtensorMap* w, const CUtensorMap* w2, const CUtensorMap* x, const GemmParams& p, cudaStream_t s,
+                         const L2Prefetch* pf) {
   switch (epi) {
     case EPI_STORE:
-      if constexpr (MPAD < 256) return launch_one_x<T, MPAD, EPI_STORE, false, true>(w, nullptr, x, x, p, s, pf);
+      if constexpr (MPAD < 256) return launch_one_x<T, MPAD, EPI_STORE, false, WQ>(w, w2, x, x, p, s, pf);
       break;
-    case EPI_RESIDUAL: return launch_one_x<T, MPAD, EPI_RESIDUAL, false, true>(w, nullptr, x, x, p, s, pf);
-    case EPI_QKV_ROPE: return launch_one_x<T, MPAD, EPI_QKV_ROPE, false, true>(w, nullptr, x, x, p, s, pf);
-    case EPI_SWIGLU_IL: return launch_one_x<T, MPAD, EPI_SWIGLU_IL, false, true>(w, nullptr, x, x, p, s, pf);
+    case EPI_RESIDUAL: return launch_one_x<T, MPAD, EPI_RESIDUAL, false, WQ>(w, w2, x, x, p, s, pf);
+    case EPI_QKV_ROPE: return launch_one_x<T, MPAD, EPI_QKV_ROPE, false, WQ>(w, w2, x, x, p, s, pf);
+    case EPI_SWIGLU_IL: return launch_one_x<T, MPAD, EPI_SWIGLU_IL, false, WQ>(w, w2, x, x, p, s, pf);
+  }
+  return static_cast<int>(cudaErrorInvalidValue);
+}
+template <int WQ>
+static int launch_wq(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, GemmParams& p,
+                     cudaStream_t s, const L2Prefetch* pf) {
+  if (epi == EPI_SWIGLU_IL) {
+    p.silu_lut = silu_lut(dtype, s);
+    if (!p.silu_lut) return static_cast<int>(cudaErrorNotReady);
+  }
+  if (dtype == DT_BF16) {
+    if (mpad == 16) return launch_wq_epi<__nv_bfloat16, 16, WQ>(epi, tmW, tmW2, tmX, p, s, pf);
+    if (mpad == 64) return launch_wq_epi<__nv_bfloat16, 64, WQ>(epi, tmW, tmW2, tmX, p, s, pf);
+    if (mpad == 256) return launch_wq_epi<__nv_bfloat16, 256, WQ>(epi, tmW, tmW2, tmX, p, s, pf);
+  } else if (dtype == DT_FP16) {
+    if (mpad == 16) return launch_wq_epi<__half, 16, WQ>(epi, tmW, tmW2, tmX, p, s, pf);
+    if (mpad == 64) return launch_wq_epi<__half, 64, WQ>(epi, tmW, tmW2, tmX, p, s, pf);
+    if (mpad == 256) return launch_wq_epi<__half, 256, WQ>(epi, tmW, tmW2, tmX, p, s, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }
@@ -530,20 +636,49 @@ int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const C
                    const L2Prefetch* pf) {
   GemmParams p = p_in;
   if (p.splitk < 1 || p.m_rows > mpad || !p.w_scale) return static_cast<int>(cudaErrorInvalidValue);
-  if (epi == EPI_SWIGLU_IL) {
-    p.silu_lut = silu_lut(dtype, s);
-    if (!p.silu_lut) return static_cast<int>(cudaErrorNotReady);
+  return launch_wq<WQ_INT8>(dtype, mpad, epi, tmW, nullptr, tmX, p, s, pf);
+}
+
+int launch_gemm_w4(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmA, const CUtensorMap* tmX, const GemmParams& p_in,
+                   cudaStream_t s, const L2Prefetch* pf) {
+  GemmParams p = p_in;
+  if (p.splitk < 1 || p.m_rows > mpad || !tmA || p.K % kBlockK || (p.w4_quant != W4_NF4 && p.w4_quant != W4_FP4))
+    return static_cast<int>(cudaErrorInvalidValue);
+  return launch_wq<WQ_4BIT>(dtype, mpad, epi, tmW, tmA, tmX, p, s, pf);
+}
+
+// one thread per source byte (nibbles) and per source absmax; see kernels.h for the layouts
+__global__ void w4_repack_kernel(const uint8_t* __restrict__ src, const float* __restrict__ src_absmax, int nr, int K, int row0, int half,
+                                 uint8_t* __restrict__ dst, float* __restrict__ dst_absmax, int n_pad) {
+  const int kbytes = K / 2, num_kb = K / kBlockK;
+  const long n_bytes = src ? static_cast<long>(nr) * kbytes : 0, n_abs = src_absmax ? static_cast<long>(nr) * num_kb : 0;
+  for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < n_bytes + n_abs; i += static_cast<long>(gridDim.x) * blockDim.x) {
+    const bool is_abs = i >= n_bytes;
+    const long j = is_abs ? i - n_bytes : i;
+    const int row = static_cast<int>(j / (is_abs ? num_kb : kbytes)), col = static_cast<int>(j % (is_abs ? num_kb : kbytes));
+    const int d = half >= 0 ? (row / 64) * 128 + half * 64 + row % 64 : row0 + row;
+    if (d >= n_pad) continue;  // the launcher checks the destination; this keeps a bad call inside the buffers
+    if (is_abs) {
+      dst_absmax[static_cast<long>(col) * n_pad + d] = src_absmax[j];
+      continue;
+    }
+    // byte b of the k-block holds K columns 2b, 2b + 1: k16 step b / 8, fragment column pair b % 4 of the low (b % 8 < 4) or high half
+    const int r = d % kBlockN, kb = col / 32, b = col % 32;
+    const int tidx = (r / 64) * 128 + ((r % 64) / 16) * 32 + (r % 8) * 4 + (b % 4);
+    const int reg = ((b % 8) / 4) * 2 + (r % 16) / 8;
+    dst[(static_cast<long>(d / kBlockN) * num_kb + kb) * kW4TileBytes + tidx * 16 + (b / 8) * 4 + reg] = src[j];
   }
-  if (dtype == DT_BF16) {
-    if (mpad == 16) return launch_w8_epi<__nv_bfloat16, 16>(epi, tmW, tmX, p, s, pf);
-    if (mpad == 64) return launch_w8_epi<__nv_bfloat16, 64>(epi, tmW, tmX, p, s, pf);
-    if (mpad == 256) return launch_w8_epi<__nv_bfloat16, 256>(epi, tmW, tmX, p, s, pf);
-  } else if (dtype == DT_FP16) {
-    if (mpad == 16) return launch_w8_epi<__half, 16>(epi, tmW, tmX, p, s, pf);
-    if (mpad == 64) return launch_w8_epi<__half, 64>(epi, tmW, tmX, p, s, pf);
-    if (mpad == 256) return launch_w8_epi<__half, 256>(epi, tmW, tmX, p, s, pf);
-  }
-  return static_cast<int>(cudaErrorInvalidValue);
+}
+int launch_w4_repack(const uint8_t* src, const float* src_absmax, int nr, int K, int row0, int half, uint8_t* dst, float* dst_absmax,
+                     int n_pad, cudaStream_t s) {
+  if (nr < 0 || K <= 0 || K % kBlockK || n_pad % kBlockN || (src && !dst) || (src_absmax && !dst_absmax)) return static_cast<int>(cudaErrorInvalidValue);
+  if (half >= 0 ? (nr % 64 || 2L * nr > n_pad) : (row0 < 0 || static_cast<long>(row0) + nr > n_pad))
+    return static_cast<int>(cudaErrorInvalidValue);  // destination rows beyond the buffers
+  const long total = (src ? static_cast<long>(nr) * (K / 2) : 0) + (src_absmax ? static_cast<long>(nr) * (K / kBlockK) : 0);
+  if (total == 0) return 0;
+  const int blocks = static_cast<int>(std::min<long>((total + 255) / 256, 8192));
+  w4_repack_kernel<<<blocks, 256, 0, s>>>(src, src_absmax, nr, K, row0, half, dst, dst_absmax, n_pad);
+  return static_cast<int>(cudaGetLastError());
 }
 
 template <typename T, int MPAD>

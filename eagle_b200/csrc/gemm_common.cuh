@@ -27,6 +27,15 @@ constexpr int kW8DqBytes = kWTileBytes;
 __host__ __device__ constexpr int stage_bytes_w8(int mpad) { return kW8TileBytes + x_tile_bytes(mpad); }
 // transformers' bnb 8-bit dequantization factor (integrations/bitsandbytes.py), as the fp32 value torch multiplies by
 constexpr float kInv127 = 7.874015718698502e-3f;
+// W4A16 (bitsandbytes nf4 / fp4 codes, one fp32 absmax per 64-element block of a row): a stage holds the 4 KB nibble tile in
+// the engine's fragment order (launch_w4_repack), the tile's 128 absmax values of the k-block, padding to 1 KB so the X tile
+// stays 1024-byte aligned, and the X tile
+constexpr int kW4TileBytes = kBlockN * kBlockK / 2;
+constexpr int kW4AbsBytes = kBlockN * 4;
+constexpr int kW4WBytes = 5 * 1024;
+__host__ __device__ constexpr int stage_bytes_w4(int mpad) { return kW4WBytes + x_tile_bytes(mpad); }
+// weight modes of skinny_gemm_wgmma
+enum WeightQuant : int { WQ_NONE = 0, WQ_INT8 = 1, WQ_4BIT = 2 };
 
 // number of SMs of the current device (the grids are sized to fill it)
 inline int device_sm_count() {

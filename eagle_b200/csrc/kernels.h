@@ -59,6 +59,7 @@ struct GemmParams {
   int m_idx;         // >= 0: additionally clamp to st[m_idx]
   const int* st;     // device state
   int splitk;
+  int w4_quant;      // launch_gemm_w4: code table of the 4-bit weights (W4_NF4 / W4_FP4); fills the padding before ws
   float* ws;         // split-K partials  [split][acc][MPAD][n_tiles*128]
   int* counters;     // per-n-tile arrival counters (self-resetting)
   // EPI_STORE / RESIDUAL / SWIGLU
@@ -109,6 +110,19 @@ int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUte
 // EPI_QKV_ROPE, EPI_SWIGLU_IL; mpad 256: the last three.
 int launch_gemm_w8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmX, const GemmParams& p, cudaStream_t s,
                    const L2Prefetch* pf = nullptr);
+// W4A16 form (bitsandbytes nf4 / fp4 with blocksize 64): tmW maps the nibble tiles written by launch_w4_repack (2-D, rows of 256 B,
+// box 256 x 16 = one 4 KB tile), tmA the transposed absmax [K/64][n_pad] (box 128 x 1).  The MMA warpgroups convert each k16 step of
+// nibbles into their wgmma A fragments, W' = T(code[q] * absmax) (one fp32 product, one round-to-nearest cast), while the previous
+// step's MMA runs, so the result is bit-identical to launch_gemm on W'.  Epilogues and mpad as launch_gemm_w8.
+enum W4Quant : int { W4_NF4 = 0, W4_FP4 = 1 };
+int launch_gemm_w4(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmA, const CUtensorMap* tmX, const GemmParams& p,
+                   cudaStream_t s, const L2Prefetch* pf = nullptr);
+// Load-time repack of bitsandbytes' 4-bit layout into the kernel's.  Source row i (of nr) of a [nr][K/2] nibble matrix (element 2j in
+// the high nibble of byte j) and of its [nr][K/64] absmax goes to destination row d(i) = row0 + i, or, for half >= 0, to the gate/up
+// interleave (i / 64) * 128 + half * 64 + i % 64.  Nibbles land in tiles [n_pad / 128][K / 64][4096 B], each thread's four k16 steps of
+// A-fragment bytes contiguous (16 B); absmax lands transposed in [K / 64][n_pad].  K % 64 == 0.
+int launch_w4_repack(const uint8_t* src, const float* src_absmax, int nr, int K, int row0, int half, uint8_t* dst, float* dst_absmax,
+                     int n_pad, cudaStream_t s);
 // bring-up / debugging aid: same epilogues, plain FMA main loop, no TMA/wgmma.  W/W2/X are raw pointers.
 int launch_gemm_simt(int dtype, int mpad, int epi, const void* W, const void* W2, const void* X, long ldx,
                      const GemmParams& p, cudaStream_t s);

@@ -20,10 +20,11 @@ from typing import Dict, Iterator, Optional
 import torch
 
 from . import _lib
-from .quant import is_target_projection, quantize_int8_rowwise
+from .quant import is_target_projection, quantize_4bit, quantize_int8_rowwise
 
 _TORCH2ENGINE = {torch.bfloat16: _lib.DT_BF16, torch.float16: _lib.DT_FP16, torch.float32: _lib.DT_FP32,
-                 torch.int64: _lib.DT_INT64, torch.bool: _lib.DT_BOOL, torch.int8: _lib.DT_INT8}
+                 torch.int64: _lib.DT_INT64, torch.bool: _lib.DT_BOOL, torch.int8: _lib.DT_INT8,
+                 torch.uint8: _lib.DT_UINT8}
 
 
 def _llama3_inv_freq(inv_freq: torch.Tensor, rs: dict, max_position_embeddings: int) -> torch.Tensor:
@@ -132,7 +133,7 @@ class EaModel(torch.nn.Module):
     def __init__(self, target_config: dict, head_config: dict, use_eagle3: bool = True, total_token: int = 60,
                  depth: int = 7, top_k: int = 10, threshold: float = 1.0, torch_dtype: torch.dtype = torch.bfloat16,
                  device: int = 0, max_length: int = 2048, tokenizer=None, flags: int = 0, tp_rank: int = 0,
-                 tp_size: int = 1, tree_choices=None, load_in_8bit: bool = False):
+                 tp_size: int = 1, tree_choices=None, load_in_8bit: bool = False, quantization_config=None):
         super().__init__()
         self.training = False
         self.lib = _lib.load()
@@ -156,8 +157,21 @@ class EaModel(torch.nn.Module):
         self.max_length = int(max_length)
         # int8 target projections (eagle_b200.quant): bitsandbytes' weight format, exact W8A16 arithmetic
         self.load_in_8bit = bool(load_in_8bit)
+        # quantization_config (a transformers BitsAndBytesConfig or its dict): load_in_4bit gives 4-bit target projections in
+        # bitsandbytes' nf4 / fp4 format with exact W4A16 arithmetic (eagle_b200.quant), load_in_8bit the int8 ones
+        from .checkpoint import quantization_config_dict, target_weights_4bit
+        qc = quantization_config_dict(quantization_config)
+        self.quant_4bit = target_weights_4bit(qc, torch_dtype)
+        if qc and not self.quant_4bit:
+            if not qc.get("load_in_8bit"):
+                raise ValueError("quantization_config: supported are bitsandbytes load_in_4bit (nf4 / fp4) and load_in_8bit")
+            self.load_in_8bit = True
+        if self.quant_4bit and self.load_in_8bit:
+            raise ValueError("load_in_8bit and a 4-bit quantization_config exclude each other")
         if self.load_in_8bit:
             flags |= _lib.FLAG_TARGET_INT8
+        if self.quant_4bit:
+            flags |= _lib.FLAG_TARGET_NF4 if self.quant_4bit == "nf4" else _lib.FLAG_TARGET_FP4
         # attributes callers touch (ea_model.py:168; evaluation scripts)
         self.ea_layer = SimpleNamespace(total_tokens=total_token - 1, depth=depth, top_k=top_k)
         self.base_model = SimpleNamespace(config=self.config, dtype=torch_dtype, device=torch.device("cuda", int(device)))
@@ -207,7 +221,7 @@ class EaModel(torch.nn.Module):
     # weights
     # ---------------------------------------------------------------------------------------------
     def _load(self, name: str, t: torch.Tensor):
-        if t.dtype.is_floating_point and t.dtype != self.dtype and not name.endswith(".SCB"):
+        if t.dtype.is_floating_point and t.dtype != self.dtype and not name.endswith((".SCB", ".absmax")):
             t = t.to(self.dtype)  # `.to(base_model.dtype)` (ea_model.py:77)
         t = t.contiguous()
         if t.is_cuda:
@@ -217,12 +231,16 @@ class EaModel(torch.nn.Module):
         _lib.check(self.lib.eb200_load_tensor(self._h, name.encode(), t.data_ptr(), shape, t.dim(), _TORCH2ENGINE[t.dtype]))
 
     def _load_target(self, name: str, t: torch.Tensor):
-        """One target tensor; with load_in_8bit a model-dtype projection weight is quantized here (eagle_b200.quant), one tensor
-        at a time, and goes in as its int8 weight + SCB pair."""
+        """One target tensor; with load_in_8bit (4-bit) a model-dtype projection weight is quantized here (eagle_b200.quant), one
+        tensor at a time, and goes in as its int8 weight + SCB pair (uint8 codes + `.weight.absmax`)."""
         if self.load_in_8bit and t.dtype.is_floating_point and name.endswith(".weight") and is_target_projection(name):
             q, scb = quantize_int8_rowwise(t.to(self.dtype))
             self._load(name, q)
             self._load(name[: -len("weight")] + "SCB", scb)
+        elif self.quant_4bit and t.dtype.is_floating_point and name.endswith(".weight") and is_target_projection(name):
+            packed, absmax = quantize_4bit(t.to(self.dtype), self.quant_4bit)
+            self._load(name, packed)
+            self._load(name + ".absmax", absmax)
         else:
             self._load(name, t)
 
@@ -289,25 +307,48 @@ class EaModel(torch.nn.Module):
         """Same signature as the reference (ea_model.py:88-170).  Reads an HF Llama checkpoint directory
         (config.json + safetensors / .bin shards) and a draft-head directory (config.json + pytorch_model.bin or
         model.safetensors).  kwargs honoured: torch_dtype, max_length, device, tree_choices, load_in_8bit (int8 target projections,
-        eagle_b200.quant; a checkpoint saved in transformers' bitsandbytes 8-bit format loads its int8 values as stored);
-        HF placement knobs (`device_map`, `low_cpu_mem_usage`) are accepted with a warning, load_in_4bit and anything else raise."""
-        from .checkpoint import iter_checkpoint_tensors, iter_int8_pairs, read_json, target_weights_int8
-        honoured = {"torch_dtype", "max_length", "device", "tree_choices", "load_in_8bit", "load_in_4bit"}
+        eagle_b200.quant; a checkpoint saved in transformers' bitsandbytes 8-bit format loads its int8 values as stored),
+        quantization_config (a BitsAndBytesConfig or its dict: load_in_4bit with nf4 / fp4 gives 4-bit target projections; a
+        checkpoint saved in transformers' bitsandbytes 4-bit format loads its codes as stored); HF placement knobs (`device_map`,
+        `low_cpu_mem_usage`) are accepted with a warning, a bare load_in_4bit and anything else raise."""
+        from .checkpoint import (check_4bit_checkpoint, iter_4bit_triples, iter_checkpoint_tensors, iter_int8_pairs,
+                                 quantization_config_dict, read_json, target_weights_4bit, target_weights_int8)
+        honoured = {"torch_dtype", "max_length", "device", "tree_choices", "load_in_8bit", "load_in_4bit", "quantization_config"}
         placement = {"device_map", "low_cpu_mem_usage"}  # HF / accelerate loading knobs
         unknown = set(kwargs) - honoured - placement
         if unknown:
             raise TypeError(f"EaModel.from_pretrained: unsupported arguments {sorted(unknown)}")
         ignored = sorted(k for k in kwargs if k in placement and kwargs[k] not in (None, False))
         if kwargs.get("load_in_4bit"):
-            target_weights_int8({}, load_in_4bit=True)  # raises, naming what is supported
+            # a bare load_in_4bit meant transformers 4.x's implicit defaults (fp4, fp32 compute) and is gone from transformers 5
+            raise ValueError("a bare load_in_4bit=True is not supported: name the 4-bit format, "
+                             "quantization_config=BitsAndBytesConfig(load_in_4bit=True, bnb_4bit_quant_type='nf4' or 'fp4')")
         if ignored:
             warnings.warn(f"eagle_b200 places the whole model on one GPU (`device`); ignoring {ignored}", stacklevel=2)
         tc = read_json(os.path.join(base_model_path, "config.json"))
         if tc.get("architectures", ["LlamaForCausalLM"])[0] != "LlamaForCausalLM":
             raise ValueError("eagle_b200 supports Llama-family targets (the configs named in BASELINE.json)")
-        int8 = target_weights_int8(tc, kwargs.get("load_in_8bit", False))
-        hc = read_json(os.path.join(ea_model_path, "config.json"))
         dtype = kwargs.get("torch_dtype", torch.float16)
+        # 4-bit first (target_weights_int8 refuses every 4-bit request): codes stored by transformers' bitsandbytes 4-bit
+        # serialization, else a 4-bit quantization_config argument
+        qc_arg = quantization_config_dict(kwargs.get("quantization_config"))
+        stored_4bit = target_weights_4bit(tc.get("quantization_config"), dtype, pre_quantized=True)
+        asked_4bit = target_weights_4bit(qc_arg, dtype, pre_quantized=bool(stored_4bit))
+        asked_8bit = bool(kwargs.get("load_in_8bit")) or bool(qc_arg.get("load_in_8bit"))
+        if asked_4bit and asked_8bit:
+            raise ValueError("load_in_8bit and a 4-bit quantization_config exclude each other")
+        if stored_4bit:
+            # the stored format decides; a request for another one is refused rather than ignored
+            if asked_8bit or (asked_4bit and asked_4bit != stored_4bit):
+                raise ValueError(f"{base_model_path} holds bitsandbytes {stored_4bit} weights; the request for "
+                                 f"{'load_in_8bit' if asked_8bit else asked_4bit} conflicts with them")
+            check_4bit_checkpoint(base_model_path, stored_4bit, dtype)
+        elif asked_4bit and tc.get("quantization_config"):
+            raise ValueError(f"{base_model_path} is already quantized (quantization_config {tc['quantization_config']}); a 4-bit "
+                             f"quantization_config applies to bf16 / fp16 checkpoints only")
+        quant_4bit = stored_4bit or asked_4bit
+        int8 = False if quant_4bit else target_weights_int8(tc, kwargs.get("load_in_8bit", False) or bool(qc_arg.get("load_in_8bit")))
+        hc = read_json(os.path.join(ea_model_path, "config.json"))
         tok = None
         try:
             from transformers import AutoTokenizer
@@ -316,13 +357,15 @@ class EaModel(torch.nn.Module):
             tok = None
         m = cls(tc, hc, use_eagle3=use_eagle3, total_token=total_token, depth=depth, top_k=top_k, threshold=threshold,
                 torch_dtype=dtype, device=kwargs.get("device", 0), max_length=kwargs.get("max_length", 2048), tokenizer=tok,
-                tree_choices=kwargs.get("tree_choices"), load_in_8bit=int8)
-        for k, v, scb in iter_int8_pairs(base_model_path):
+                tree_choices=kwargs.get("tree_choices"), load_in_8bit=int8,
+                quantization_config={"load_in_4bit": True, "bnb_4bit_quant_type": quant_4bit} if quant_4bit else None)
+        triples = iter_4bit_triples(base_model_path, stored_4bit, dtype) if stored_4bit else iter_int8_pairs(base_model_path)
+        for k, v, aux in triples:
             if "rotary_emb" in k:
                 continue
-            if scb is not None:  # stored bitsandbytes int8: loaded as is, not requantized
+            if aux is not None:  # stored bitsandbytes int8 / 4-bit: loaded as is, not requantized
                 m._load(k, v)
-                m._load(k[: -len("weight")] + "SCB", scb)
+                m._load(k + ".absmax" if stored_4bit else k[: -len("weight")] + "SCB", aux)
             else:
                 m._load_target(k, v)
         head_sd = dict(iter_checkpoint_tensors(ea_model_path, prefer_bin=True))

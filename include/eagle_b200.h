@@ -25,10 +25,10 @@
 extern "C" {
 #endif
 
-#define EB200_ABI_VERSION 2
+#define EB200_ABI_VERSION 3
 
 enum { EB200_BF16 = 0, EB200_FP16 = 1 };
-enum { EB200_DT_BF16 = 0, EB200_DT_FP16 = 1, EB200_DT_FP32 = 2, EB200_DT_INT64 = 3, EB200_DT_BOOL = 4, EB200_DT_INT8 = 5 };
+enum { EB200_DT_BF16 = 0, EB200_DT_FP16 = 1, EB200_DT_FP32 = 2, EB200_DT_INT64 = 3, EB200_DT_BOOL = 4, EB200_DT_INT8 = 5, EB200_DT_UINT8 = 6 };
 
 typedef struct eb200_engine eb200_engine;
 
@@ -67,6 +67,13 @@ typedef struct eb200_config {
  * Single GPU, default GEMM path only: eb200_finalize refuses tp_size > 1, EB200_FLAG_SIMT_GEMM, EB200_CHAIN=1 and
  * EB200_GEMM_MODE=streamk. */
 #define EB200_FLAG_TARGET_INT8 8
+/* The same projections stored as bitsandbytes 4-bit codes (NF4 or FP4 table, blocksize 64: one fp32 absmax per 64 consecutive
+ * elements of a row) and multiplied by a W4A16 GEMM that computes exactly what the model-dtype GEMM computes on
+ * W' = dtype(code[q] * absmax) (one fp32 product, one round-to-nearest cast).  The two flags exclude each other and
+ * EB200_FLAG_TARGET_INT8; the in-features of every projection must be a multiple of 64.  Same restrictions as int8, and
+ * eb200_create already refuses them with tp_size > 1 (the loader places whole tensors). */
+#define EB200_FLAG_TARGET_NF4 16
+#define EB200_FLAG_TARGET_FP4 32
 
 typedef struct eb200_gen_params {
   float temperature, top_p;   /* eagenerate(temperature, top_p, top_k, ...) ea_model.py:199-208 */
@@ -96,7 +103,10 @@ void eb200_destroy(eb200_engine* e);
  * this rank's shard.  shape has ndim entries.
  * EB200_FLAG_TARGET_INT8 engines take each target projection as "model.layers.{i}.<proj>.weight" in EB200_DT_INT8 [out, in]
  * plus "model.layers.{i}.<proj>.SCB" in EB200_DT_FP32 [out] (its row absmax, the key transformers serializes bnb 8-bit models
- * with); model-dtype data for those names is rejected, and so is int8 data anywhere else or for an engine without the flag. */
+ * with); model-dtype data for those names is rejected, and so is int8 data anywhere else or for an engine without the flag.
+ * EB200_FLAG_TARGET_NF4 / _FP4 engines take "model.layers.{i}.<proj>.weight" in EB200_DT_UINT8 [out, in / 2] (bitsandbytes' packing:
+ * element 2j in the high nibble of byte j) plus "model.layers.{i}.<proj>.weight.absmax" in EB200_DT_FP32 [out, in / 64]; the engine
+ * repacks both on the device into its kernel's private layout. */
 int eb200_load_tensor(eb200_engine* e, const char* name, const void* data, const int64_t* shape, int32_t ndim,
                       int32_t dtype);
 /* cos/sin tables [n_pos][head_dim/2] in the model dtype, built by the caller exactly like the reference's
@@ -205,6 +215,10 @@ int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const void* W, c
  * eb200_k_gemm (0 store, 1 residual, 5 interleaved SwiGLU with N output columns over a [2N, K] weight); bias: store only */
 int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, const void* scb, const void* X, void* out, const void* res,
                     const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
+/* the W4A16 GEMM (EB200_FLAG_TARGET_NF4 / _FP4) on bitsandbytes' layout: Wq uint8 [N, K/2], absmax fp32 [N, K/64], quant_type
+ * 0 = nf4, 1 = fp4; the engine's load-time repack is applied first.  Epilogues and M as eb200_k_gemm_w8; K % 64 == 0. */
+int eb200_k_gemm_w4(int32_t dtype, int32_t quant_type, int32_t epilogue, const void* Wq, const void* absmax, const void* X, void* out,
+                    const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
 /* micro-benchmark of the skinny GEMM: `iters` back-to-back launches cycling over `n_weights` distinct [N,K] weight
  * matrices (so the stream is HBM-, not L2-resident), timed with CUDA events; optionally replayed from a CUDA graph.
  * epilogue: 0 store, 1 residual, 2 swiglu.  Returns the average microseconds per launch. */
