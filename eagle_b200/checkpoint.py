@@ -11,6 +11,7 @@ from __future__ import annotations
 import glob
 import json
 import os
+import re
 from typing import Iterator, Optional, Tuple
 
 import torch
@@ -283,6 +284,82 @@ def bnb_4bit_entries(name: str, w: torch.Tensor, quant_type: str, double_quant: 
     return out
 
 
+def target_weights_fp8(quantization_config, num_layers: int = 1) -> bool:
+    """Whether a quantization_config (transformers' FineGrainedFP8Config or its dict, or a checkpoint's `quantization_config`)
+    asks for FP8 target projections.  Honoured: `quant_method` "fp8" with `weight_block_size` [128, 128] (transformers' default
+    when absent) and `activation_scheme` "dynamic": the engine multiplies by the dequantized W' in the model dtype, so only the
+    weight format matters.  Raises ValueError for what it cannot honour: a static activation scheme (its checkpoints carry
+    `activation_scale` tensors the model-dtype arithmetic would ignore), any other block size or a per-tensor scale
+    (`weight_block_size: null`), `dequantize: true`, and a `modules_to_not_convert` that names a decoder projection of one of
+    the `num_layers` layers (transformers' should_convert_module rule)."""
+    qc = quantization_config_dict(quantization_config)
+    method = qc.get("quant_method")
+    if getattr(method, "value", method) != "fp8":
+        return False
+    scheme = str(qc.get("activation_scheme") or "dynamic").lower()
+    if scheme != "dynamic":
+        raise ValueError(f"FP8 activation_scheme={scheme!r} is not supported: static schemes carry activation_scale tensors; "
+                         f"the engine loads dynamic-scheme FP8 weights and multiplies by them in the model dtype")
+    block = qc.get("weight_block_size", (128, 128))
+    if block is None or [int(v) for v in block] != [128, 128]:
+        raise ValueError(f"FP8 weight_block_size={block!r} is not supported: the engine reads one scale per 128 x 128 block "
+                         f"(FineGrainedFP8Config's default)")
+    if qc.get("dequantize"):
+        raise ValueError("FP8 dequantize=True is not supported: load the dequantized bf16 / fp16 checkpoint instead")
+    from .quant import PROJECTIONS
+    for key in qc.get("modules_to_not_convert") or ():
+        for i in range(max(1, int(num_layers))):
+            for proj in PROJECTIONS:
+                name = f"model.layers.{i}.{proj}"
+                if re.match(f"{key}\\.", name) or re.match(f"{key}", name) or name.endswith(key):
+                    raise ValueError(f"FP8 modules_to_not_convert entry {key!r} keeps the decoder projection {name} unquantized; the "
+                                     f"engine stores every decoder projection in FP8 or none")
+    return True
+
+
+def fp8_config_dict() -> dict:
+    """The quantization_config transformers writes for FineGrainedFP8Config() (lm_head stays in the model dtype)."""
+    return {"quant_method": "fp8", "activation_scheme": "dynamic", "weight_block_size": [128, 128], "dequantize": False,
+            "modules_to_not_convert": ["lm_head"]}
+
+
+def iter_fp8_pairs(directory: str) -> Iterator[Tuple[str, torch.Tensor, Optional[torch.Tensor]]]:
+    """Tensors of a target checkpoint saved in transformers' fine-grained FP8 format as (name, tensor, weight_scale_inv): an FP8
+    projection's float8_e4m3fn `weight` comes with its fp32 [out / 128, in / 128] `weight_scale_inv`, every other tensor with None.
+    Streamed like iter_int8_pairs.  Refused with ValueError: FP8 weights outside the decoder projections, `activation_scale`
+    tensors (static activation schemes), a scale whose shape does not tile its weight in 128 x 128 blocks, unpaired entries."""
+    from .quant import FP8_BLOCK, is_target_projection
+    weights, scales = {}, {}
+
+    def pair(name, q, s):
+        n, k = q.shape
+        if n % FP8_BLOCK or k % FP8_BLOCK or tuple(s.shape) != (n // FP8_BLOCK, k // FP8_BLOCK):
+            raise ValueError(f"{name}: weight [{n}, {k}] and weight_scale_inv {list(s.shape)} are not one scale per 128 x 128 block")
+        return name, q, s
+
+    for k, v in iter_checkpoint_tensors(directory):
+        if k.endswith(".activation_scale"):
+            raise ValueError(f"{k}: static FP8 activation scales are not supported (activation_scheme 'dynamic' only)")
+        if k.endswith(".weight_scale_inv"):
+            base = k[: -len("weight_scale_inv")]
+            if base in weights:
+                yield pair(base + "weight", weights.pop(base), v)
+            else:
+                scales[base] = v
+        elif v.dtype == torch.float8_e4m3fn:
+            if not (k.endswith(".weight") and is_target_projection(k)):
+                raise ValueError(f"{k}: FP8 weights are supported for the target decoder projections only")
+            base = k[: -len("weight")]
+            if base in scales:
+                yield pair(k, v, scales.pop(base))
+            else:
+                weights[base] = v
+        else:
+            yield k, v, None
+    if weights or scales:
+        raise ValueError(f"FP8 checkpoint {directory}: unpaired weight / weight_scale_inv entries {sorted(list(weights) + list(scales))[:4]}")
+
+
 def save_head_checkpoint(directory: str, head_config: dict, head_sd: dict, as_bin: bool = False):
     """Write a draft-head directory in the reference's format (config.json + weights)."""
     os.makedirs(directory, exist_ok=True)
@@ -297,12 +374,24 @@ def save_head_checkpoint(directory: str, head_config: dict, head_sd: dict, as_bi
 
 
 def save_target_checkpoint(directory: str, target_config: dict, target_sd: dict, load_in_4bit: Optional[str] = None,
-                           double_quant: bool = False):
+                           double_quant: bool = False, fp8: bool = False):
     """HF Llama directory (config.json + model.safetensors).  A state dict holding int8 `weight` + `SCB` pairs is saved the
     way transformers saves a bitsandbytes 8-bit model: add `quantization_config` with `load_in_8bit: true` to the config.
     load_in_4bit="nf4" | "fp4" saves the model-dtype decoder projections of `target_sd` in bitsandbytes' 4-bit format instead
-    (bnb_4bit_entries, double-quantized absmax with double_quant) and adds the matching `quantization_config`."""
+    (bnb_4bit_entries, double-quantized absmax with double_quant) and adds the matching `quantization_config`.  fp8=True saves
+    them in transformers' fine-grained FP8 format (quant.quantize_fp8_block: float8_e4m3fn `weight` + fp32 `weight_scale_inv`)
+    with FineGrainedFP8Config's `quantization_config`."""
     os.makedirs(directory, exist_ok=True)
+    if fp8:
+        from .quant import is_target_projection, quantize_fp8_block
+        sd = {}
+        for k, v in target_sd.items():
+            if k.endswith(".weight") and v.dtype.is_floating_point and is_target_projection(k):
+                sd[k], sd[k[: -len("weight")] + "weight_scale_inv"] = quantize_fp8_block(v)
+            else:
+                sd[k] = v
+        target_sd = sd
+        target_config = {**target_config, "quantization_config": fp8_config_dict()}
     if load_in_4bit:
         from .quant import is_target_projection
         sd = {}

@@ -117,21 +117,36 @@ static int make_tmap_w4(CUtensorMap* w, CUtensorMap* a, const void* tiles, const
                                      (unsigned long long)K);
   return 0;
 }
+// FP8 (launch_gemm_fp8): the repacked e4m3 [N][K] maps like an int8 weight; the block scales [N / 128][K / 128][4] fp32, box = the
+// 16 B of one tile and 128-column block
+static int make_tmap_fp8(CUtensorMap* w, CUtensorMap* sc, const void* q, const float* scales, uint64_t N, uint64_t K) {
+  TRY(make_tmap_w8(w, q, N, K));
+  const cuuint64_t dims[2] = {K / 128 * 4, N / 128}, strides[1] = {K / 128 * 16};
+  const cuuint32_t box[2] = {4, 1}, es[2] = {1, 1};
+  const CUresult r = g_encode(sc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(scales), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (fp8 scales) failed (%d) N=%llu K=%llu", (int)r, (unsigned long long)N,
+                                     (unsigned long long)K);
+  return 0;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // engine data
 // ------------------------------------------------------------------------------------------------------------
+// the flags that store the target's decoder projections quantized (one at a time)
+constexpr int kTargetQuantFlags = EB200_FLAG_TARGET_INT8 | EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4 | EB200_FLAG_TARGET_FP8;
 struct Linear {
   void* w = nullptr;
   int N = 0, K = 0;
-  int esize = 2;              // bytes per weight: 2 (model dtype) or 1 (int8, EB200_FLAG_TARGET_INT8)
+  int esize = 2;              // bytes per weight: 2 (model dtype) or 1 (int8 / FP8, EB200_FLAG_TARGET_INT8 / _FP8)
   float* scale = nullptr;     // int8 only: fp32 scale of each row (SCB)
   float* absmax = nullptr;    // 4-bit only: w holds the repacked nibble tiles, absmax [K/64][n_pad] (launch_w4_repack)
   int w4_quant = -1;          // 4-bit only: W4_NF4 / W4_FP4
   int n_pad = 0;              // 4-bit only: N rounded up to whole 128-row tiles
-  CUtensorMap tm, tm_abs;     // tm_abs: 4-bit only
+  float* scale_inv = nullptr; // FP8 only: w holds the repacked e4m3 [N][K], scale_inv the block scales [N/128][K/128][4] (launch_fp8_repack)
+  CUtensorMap tm, tm_abs;     // tm_abs: the 4-bit absmax / FP8 block scales
   uint64_t loaded_rows = 0;   // bookkeeping for fused / sharded loads
-  uint64_t loaded_scales = 0; // int8 SCB / 4-bit absmax
+  uint64_t loaded_scales = 0; // int8 SCB / 4-bit absmax / FP8 weight_scale_inv
 };
 struct ActBuf {  // an activation buffer usable as the X operand of the GEMM (64 rows; 256 where the prompt prefill runs through it)
   void* p = nullptr;
@@ -294,10 +309,16 @@ static int dalloc(eb200_engine* e, void** p, size_t bytes, bool zero = true) {
   if (zero) CK(cudaMemsetAsync(*p, 0, bytes, e->stream));
   return 0;
 }
-// wq: 0 model dtype, EB200_FLAG_TARGET_INT8 / _NF4 / _FP4
+// wq: 0 model dtype, EB200_FLAG_TARGET_INT8 / _NF4 / _FP4 / _FP8
 static int alloc_linear(eb200_engine* e, Linear& l, int N, int K, int wq = 0) {
   l.N = N;
   l.K = K;
+  if (wq == EB200_FLAG_TARGET_FP8) {
+    if (N % 128 || K % 128) return fail("FP8 target weights need out- and in-features divisible by 128 (128 x 128 scale blocks), got [%d, %d]", N, K);
+    l.esize = 1;
+    TRY(dalloc(e, reinterpret_cast<void**>(&l.scale_inv), static_cast<size_t>(N / 128) * (K / 128) * 16));
+    return dalloc(e, &l.w, static_cast<size_t>(N) * K, false);
+  }
   if (wq == EB200_FLAG_TARGET_NF4 || wq == EB200_FLAG_TARGET_FP4) {
     if (K % 64) return fail("4-bit target weights need in-features divisible by 64 (blocksize 64 blocks must not straddle rows), got %d", K);
     l.w4_quant = wq == EB200_FLAG_TARGET_NF4 ? W4_NF4 : W4_FP4;
@@ -345,12 +366,16 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
   if (c.num_heads % c.tp_size || c.num_kv_heads % c.tp_size || c.intermediate_size % c.tp_size)
     return fail("heads / kv heads / intermediate size must divide by tp_size");
   {
-    const int wq = c.flags & (EB200_FLAG_TARGET_INT8 | EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4);
-    if (wq & (wq - 1)) return fail("EB200_FLAG_TARGET_INT8, EB200_FLAG_TARGET_NF4 and EB200_FLAG_TARGET_FP4 exclude each other");
-    // the 4-bit loader places whole checkpoint tensors (no tensor-parallel sharding of codes or absmax)
+    const int wq = c.flags & kTargetQuantFlags;
+    if (wq & (wq - 1))
+      return fail("EB200_FLAG_TARGET_INT8, EB200_FLAG_TARGET_NF4, EB200_FLAG_TARGET_FP4 and EB200_FLAG_TARGET_FP8 exclude each other");
+    // the 4-bit and FP8 loaders place whole checkpoint tensors (no tensor-parallel sharding of codes, absmax or block scales)
     if ((wq & (EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4)) && c.tp_size > 1)
       return fail("4-bit target weights (EB200_FLAG_TARGET_NF4 / _FP4) are not supported with tensor parallelism (tp_size %d); "
                   "they run on one GPU", c.tp_size);
+    if ((wq & EB200_FLAG_TARGET_FP8) && c.tp_size > 1)
+      return fail("FP8 target weights (EB200_FLAG_TARGET_FP8) are not supported with tensor parallelism (tp_size %d); they run on one GPU",
+                  c.tp_size);
   }
   if (c.total_token < 2 || c.total_token > 64) return fail("total_token must be in [2, 64]");
   if (c.top_k < 1 || c.top_k > 16) return fail("top_k must be in [1, 16]");
@@ -419,7 +444,7 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
     // ---- target weights
     TRY(dalloc(e, &e->t_embed, static_cast<size_t>(e->V) * H * 2, false));
     e->tl.resize(e->L);
-    const int wq = c.flags & (EB200_FLAG_TARGET_INT8 | EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4);
+    const int wq = c.flags & kTargetQuantFlags;
     for (auto& l : e->tl) {
       TRY(alloc_linear(e, l.qkv, (e->nh_l + 2 * e->nkv_l) * 128, H, wq));
       TRY(alloc_linear(e, l.o, H, e->nh_l * 128, wq));
@@ -691,19 +716,37 @@ static bool ends_with(const std::string& s, const char* suf) {
   return s.size() >= n && s.compare(s.size() - n, n, suf) == 0;
 }
 // the seven decoder-layer projections: weight "<proj>.weight"; int8 row scales "<proj>.SCB" (EB200_FLAG_TARGET_INT8); 4-bit block
-// absmax "<proj>.weight.absmax" (EB200_FLAG_TARGET_NF4 / _FP4)
+// absmax "<proj>.weight.absmax" (EB200_FLAG_TARGET_NF4 / _FP4); FP8 block scales "<proj>.weight_scale_inv" (EB200_FLAG_TARGET_FP8)
 static const char* const kProjNames[7] = {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj",
                                           "mlp.gate_proj",    "mlp.up_proj",      "mlp.down_proj"};
-enum ProjPart { PART_WEIGHT = 0, PART_SCB = 1, PART_ABSMAX = 2 };
+enum ProjPart { PART_WEIGHT = 0, PART_SCB = 1, PART_ABSMAX = 2, PART_SCALE_INV = 3 };
 static int proj_index(const std::string& sub, int* part) {
   for (int i = 0; i < 7; ++i) {
     const std::string p(kProjNames[i]);
-    if (sub == p + ".weight" || sub == p + ".SCB" || sub == p + ".weight.absmax") {
-      *part = sub == p + ".weight" ? PART_WEIGHT : sub == p + ".SCB" ? PART_SCB : PART_ABSMAX;
+    if (sub == p + ".weight" || sub == p + ".SCB" || sub == p + ".weight.absmax" || sub == p + ".weight_scale_inv") {
+      *part = sub == p + ".weight" ? PART_WEIGHT : sub == p + ".SCB" ? PART_SCB : sub == p + ".weight.absmax" ? PART_ABSMAX : PART_SCALE_INV;
       return i;
     }
   }
   return -1;
+}
+// FP8: copy the e4m3 [nr][K] tensor (or its [nr / 128][K / 128] fp32 scales) to the device and repack it into the engine's layout
+static int load_fp8(eb200_engine* e, Linear& L, bool scales, const void* data, long nr, long row0, int half) {
+  const long rows_needed = half >= 0 ? nr * 2 : row0 + nr;  // gate/up: the two halves interleave over 2 * nr rows
+  if (nr < 0 || nr % 128 || row0 < 0 || row0 % 64 || rows_needed > L.N)
+    return fail("FP8 load: %ld source rows at destination row %ld do not fit the %d rows of the projection in 128-row blocks", nr, row0, L.N);
+  const size_t bytes = scales ? static_cast<size_t>(nr / 128) * (L.K / 128) * 4 : static_cast<size_t>(nr) * L.K;
+  void* tmp = nullptr;
+  CK(cudaMalloc(&tmp, bytes));
+  int rc = 0;
+  if (cudaMemcpyAsync(tmp, data, bytes, cudaMemcpyDefault, e->stream) != cudaSuccess) rc = fail("FP8 load: copy failed");
+  else if (launch_fp8_repack(scales ? nullptr : static_cast<const uint8_t*>(tmp), scales ? static_cast<const float*>(tmp) : nullptr,
+                             static_cast<int>(nr), L.K, static_cast<int>(row0), half, static_cast<uint8_t*>(L.w), L.scale_inv, L.N,
+                             e->stream) != 0 ||
+           cudaStreamSynchronize(e->stream) != cudaSuccess)
+    rc = fail("FP8 load: repack failed");
+  cudaFree(tmp);
+  return rc;
 }
 // 4-bit: copy the [nr][C] tensor (nibbles, or absmax with C = K / 64) to the device and repack its rows into the engine's layout
 static int load_w4(eb200_engine* e, Linear& L, bool absmax, const void* data, long nr, long row0, int half) {
@@ -750,7 +793,20 @@ static int load_layer_tensor(eb200_engine* e, Layer& l, const std::string& sub, 
     const std::string wname = std::string(kProjNames[pi]) + ".weight";
     const Shard sh = shard_of(wname, sl.rows, sl.cols, rk, tp);
     Linear& L = *sl.lin;
-    if (L.absmax) {  // 4-bit (one GPU: the shard is the whole tensor)
+    if (L.scale_inv) {  // FP8 (one GPU: the shard is the whole tensor)
+      if (part == PART_SCB || part == PART_ABSMAX)
+        return fail("%s%s: belongs to int8 / 4-bit projections; this engine stores FP8 weights", short_name, part == PART_SCB ? ".SCB" : ".weight.absmax");
+      const bool si = part == PART_SCALE_INV;
+      if (sl.rows % 128 || sl.cols % 128)
+        return fail("%s: FP8 weights need out- and in-features divisible by 128, got [%ld, %ld]", short_name, sl.rows, sl.cols);
+      if (!shape_is(shape, nd, si ? sl.rows / 128 : sl.rows, si ? sl.cols / 128 : sl.cols))
+        return fail("%s%s shape mismatch (want [%ld, %ld] %s)", short_name, si ? ".weight_scale_inv" : ".weight", si ? sl.rows / 128 : sl.rows,
+                    si ? sl.cols / 128 : sl.cols, si ? "fp32: one scale per 128 x 128 block" : "float8_e4m3fn");
+      TRY(load_fp8(e, L, si, data, sl.rows, sl.row0, sl.half));
+      (si ? L.loaded_scales : L.loaded_rows) |= sl.bit;
+    } else if (part == PART_SCALE_INV) {
+      return fail("%s.weight_scale_inv: block scales belong to FP8 projections (EB200_FLAG_TARGET_FP8)", short_name);
+    } else if (L.absmax) {  // 4-bit (one GPU: the shard is the whole tensor)
       if (part == PART_SCB) return fail("%s.SCB: row scales belong to int8 projections; this engine stores 4-bit weights", short_name);
       const bool am = part == PART_ABSMAX;
       if (!shape_is(shape, nd, sl.rows, am ? sl.cols / 64 : sl.cols / 2))
@@ -806,7 +862,20 @@ extern "C" int eb200_load_tensor(eb200_engine* e, const char* name_c, const void
   const bool scb = part == PART_SCB;
   const bool w8 = (c.flags & EB200_FLAG_TARGET_INT8) != 0;
   const bool w4 = (c.flags & (EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4)) != 0;
-  if (dtype == EB200_DT_UINT8 || ends_with(name, ".absmax")) {
+  const bool f8 = (c.flags & EB200_FLAG_TARGET_FP8) != 0;
+  if (dtype == EB200_DT_FP8_E4M3 || ends_with(name, ".weight_scale_inv")) {
+    // FP8 target projections: "<proj>.weight" float8_e4m3fn + "<proj>.weight_scale_inv" fp32 (transformers' FineGrainedFP8Config keys)
+    if (!target_proj)
+      return fail("tensor '%s': FP8 weights and weight_scale_inv are accepted only for the target decoder projections "
+                  "(q/k/v/o/gate/up/down_proj); embeddings, norms, lm_head and the draft head stay in the model dtype", name_c);
+    if (!f8) return fail("tensor '%s': FP8 data for an engine created without EB200_FLAG_TARGET_FP8", name_c);
+    if (part == PART_SCALE_INV && dtype != EB200_DT_FP32) return fail("tensor '%s': FP8 weight_scale_inv must be fp32", name_c);
+    if (part != PART_SCALE_INV && (part != PART_WEIGHT || dtype != EB200_DT_FP8_E4M3))
+      return fail("tensor '%s': FP8 data is accepted as '<proj>.weight' (float8_e4m3fn) and '<proj>.weight_scale_inv' (fp32)", name_c);
+  } else if (f8 && target_proj) {
+    return fail("tensor '%s': this engine stores the target projections in FP8 (EB200_FLAG_TARGET_FP8): pass the float8_e4m3fn weight and "
+                "its fp32 weight_scale_inv (eagle_b200.quant.quantize_fp8_block)", name_c);
+  } else if (dtype == EB200_DT_UINT8 || ends_with(name, ".absmax")) {
     // 4-bit target projections: "<proj>.weight" uint8 + "<proj>.weight.absmax" fp32
     if (!target_proj)
       return fail("tensor '%s': 4-bit codes and absmax are accepted only for the target decoder projections (q/k/v/o/gate/up/down_proj); "
@@ -931,6 +1000,10 @@ extern "C" int eb200_set_rope_table(eb200_engine* e, int32_t which, const void* 
 
 static int finalize_linear(eb200_engine* e, Linear& l, const char* what, uint64_t need) {
   if (l.loaded_rows != need) return fail("weights missing for %s", what);
+  if (l.scale_inv) {
+    if (l.loaded_scales != need) return fail("block scales missing for %s (FP8 weights need their fp32 .weight_scale_inv)", what);
+    return make_tmap_fp8(&l.tm, &l.tm_abs, l.w, l.scale_inv, l.N, l.K);
+  }
   if (l.absmax) {
     if (l.loaded_scales != need) return fail("block absmax missing for %s (4-bit weights need their fp32 .weight.absmax)", what);
     return make_tmap_w4(&l.tm, &l.tm_abs, l.w, l.absmax, l.n_pad, l.K);
@@ -946,9 +1019,10 @@ static int gemm_mode();
 extern "C" int eb200_finalize(eb200_engine* e) {
   if (!e) return fail("eb200_finalize: null engine");
   CK(cudaSetDevice(e->c.device));
-  if (e->c.flags & (EB200_FLAG_TARGET_INT8 | EB200_FLAG_TARGET_NF4 | EB200_FLAG_TARGET_FP4)) {
+  if (e->c.flags & kTargetQuantFlags) {
     // the W8A16 / W4A16 GEMMs exist as the cluster split-K kernel of one GPU only
-    const char* fmt = (e->c.flags & EB200_FLAG_TARGET_INT8) ? "int8 target weights (EB200_FLAG_TARGET_INT8)"
+    const char* fmt = (e->c.flags & EB200_FLAG_TARGET_INT8)  ? "int8 target weights (EB200_FLAG_TARGET_INT8)"
+                      : (e->c.flags & EB200_FLAG_TARGET_FP8) ? "FP8 target weights (EB200_FLAG_TARGET_FP8)"
                                                              : "4-bit target weights (EB200_FLAG_TARGET_NF4 / _FP4)";
     const char* what = nullptr;
     const char* chain = getenv("EB200_CHAIN");
@@ -1162,7 +1236,8 @@ static L2Prefetch l2_plan(const eb200_engine* e, const Linear& next, int mpad, i
   L2Prefetch pf;
   memset(&pf, 0, sizeof(pf));
   pf.j0 = pf.j1 = j0;
-  // 4-bit weights are not prefetched: their tiles and absmax are two maps with other boxes than the plan's
+  // 4-bit weights are not prefetched: their tiles and absmax are two maps with other boxes than the plan's.  FP8 weights are: their
+  // map has the int8 box (128 rows x 64 bytes, esize 1); their block scales (1/512 of the bytes) are not.
   if (!l2_prefetch_on() || !next.w || next.absmax || next.N <= 0 || next.K <= 0 || bytes <= 0) return pf;
   pf.tm = next.tm;
   pf.n_tiles = (next.N + 127) / 128;
@@ -1202,9 +1277,11 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
   if ((p.N + 127) / 128 > 8192) return fail("too many n tiles");
   p.w_scale = g.W->scale;
   p.w4_quant = g.W->w4_quant;
-  // algorithmic weight bytes: int8 weights stream N*K bytes plus the N fp32 row scales; 4-bit ones N*K/2 plus N*K/64 fp32 absmax
+  // algorithmic weight bytes: int8 weights stream N*K bytes plus the N fp32 row scales; 4-bit ones N*K/2 plus N*K/64 fp32 absmax;
+  // FP8 ones N*K plus 16 B of block scales per 128 x 128 block
   const double nk = static_cast<double>(p.N) * p.K;
-  const double bytes = g.W->absmax ? nk / 2 + 4.0 * nk / 64 : p.w_scale ? nk + 4.0 * p.N : nk * 2 * (g.epi == EPI_SWIGLU ? 2 : 1);
+  const double bytes = g.W->absmax ? nk / 2 + 4.0 * nk / 64 : p.w_scale ? nk + 4.0 * p.N : g.W->scale_inv ? nk + 16.0 * nk / (128 * 128)
+                                                                                                          : nk * 2 * (g.epi == EPI_SWIGLU ? 2 : 1);
   const char* kname = g.epi == EPI_STORE ? "gemm_store" : g.epi == EPI_RESIDUAL ? "gemm_residual" :
                       (g.epi == EPI_SWIGLU || g.epi == EPI_SWIGLU_IL) ? "gemm_swiglu" : "gemm_qkv_rope";
   {
@@ -1213,7 +1290,11 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
     if (skip_kernel(kname) || skip_kernel(kk)) return 0;
   }
   ProfScope ps(e, 0, bytes, kname);
-  if (g.W->absmax) {
+  if (g.W->scale_inv) {
+    if (cx.mpad == 256 && g.X->rows < 256) return fail("256-row GEMM on a 64-row activation buffer");
+    CKL(launch_gemm_fp8(e->dtype, cx.mpad, g.epi, &g.W->tm, &g.W->tm_abs, cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256),
+                        p, e->stream, g.pf));
+  } else if (g.W->absmax) {
     if (cx.mpad == 256 && g.X->rows < 256) return fail("256-row GEMM on a 64-row activation buffer");
     CKL(launch_gemm_w4(e->dtype, cx.mpad, g.epi, &g.W->tm, &g.W->tm_abs, cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256),
                        p, e->stream, g.pf));
@@ -2939,6 +3020,49 @@ extern "C" int eb200_k_gemm_w4(int32_t dtype, int32_t quant_type, int32_t epilog
     if (r != 0) rc = fail("eb200_k_gemm_w4: launch failed (%d)", r);
   }
   if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = fail("eb200_k_gemm_w4: %s", cudaGetErrorString(cudaGetLastError()));
+  cudaFree(buf);
+  return rc;
+}
+
+extern "C" int eb200_k_gemm_fp8(int32_t dtype, int32_t epilogue, const void* Wq, const void* scale_inv, const void* X, void* out,
+                                const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream) {
+  if (M < 1 || M > 64 || (epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !scale_inv || splitk < 1 ||
+      splitk > 8 || N < 1 || K < 128 || K % 128)
+    return fail("eb200_k_gemm_fp8: bad arguments");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const int mpad = M <= 16 ? 16 : 64;
+  const int n_out = N;  // EPI_SWIGLU_IL: Wq is the [2N, K] interleaved gate/up matrix, out is [M, N]
+  if (epilogue == EPI_SWIGLU_IL) N *= 2;
+  if (N % 128) return fail("eb200_k_gemm_fp8: the weight's rows (%d) must be a multiple of 128", N);
+  GemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.N = N;
+  p.K = K;
+  p.m_rows = M;
+  p.m_idx = -1;
+  p.splitk = splitk;
+  p.out = out;
+  p.ld_out = n_out;
+  p.res = res;
+  p.ld_res = n_out;
+  p.bias = bias;
+  const size_t w_bytes = static_cast<size_t>(N) * K, s_bytes = static_cast<size_t>(N / 128) * (K / 128) * 16;
+  void* buf = nullptr;
+  CK(cudaMalloc(&buf, w_bytes + s_bytes));
+  uint8_t* q = static_cast<uint8_t*>(buf);
+  float* sc = reinterpret_cast<float*>(q + w_bytes);
+  int rc = 0;
+  CUtensorMap tw, ts, tx;
+  if (cudaMemsetAsync(sc, 0, s_bytes, s) != cudaSuccess ||
+      launch_fp8_repack(static_cast<const uint8_t*>(Wq), static_cast<const float*>(scale_inv), N, K, 0, -1, q, sc, N, s) != 0)
+    rc = fail("eb200_k_gemm_fp8: repack failed");
+  if (!rc) rc = make_tmap_fp8(&tw, &ts, q, sc, N, K);
+  if (!rc) rc = make_tmap(&tx, dtype, X, 64, K, mpad);
+  if (!rc) {
+    const int r = launch_gemm_fp8(dtype, mpad, epilogue, &tw, &ts, &tx, p, s);
+    if (r != 0) rc = fail("eb200_k_gemm_fp8: launch failed (%d)", r);
+  }
+  if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = fail("eb200_k_gemm_fp8: %s", cudaGetErrorString(cudaGetLastError()));
   cudaFree(buf);
   return rc;
 }

@@ -52,6 +52,7 @@ static int stage_count_for(int mpad, int epi, int total_ctas, int wq = WQ_NONE) 
   const int budget = mpad >= 256 ? 200 * 1024 : smem_budget(total_ctas);
   int s = wq == WQ_INT8   ? (budget - kCtrlBytes - 1024 - kW8DqBytes) / stage_bytes_w8(mpad)
           : wq == WQ_4BIT ? (budget - kCtrlBytes - 1024) / stage_bytes_w4(mpad)
+          : wq == WQ_FP8  ? (budget - kCtrlBytes - 1024) / stage_bytes_fp8(mpad)
                           : (budget - kCtrlBytes - 1024) / stage_bytes(mpad, epi);
   if (s > kMaxStages) s = kMaxStages;
   if (s < 2) s = 2;
@@ -129,6 +130,20 @@ __device__ __forceinline__ void w4_fragment(uint32_t w, uint32_t lut, float s0, 
   }
 }
 
+// W8A16 on FP8: one k16 step of a thread's A fragment from its 8 repacked e4m3 bytes (w0: registers 0, 1; w1: registers 2, 3; the
+// low byte of each half-word is the lower K column): T(fp32(q) * scale) with one __fmul_rn.  e4m3 -> f16 -> f32 is exact, so this is
+// transformers' `quantized.to(fp32) * scale_inv` followed by the model-dtype cast.  sc: the scale of the warpgroup's 64-row group.
+template <typename T>
+__device__ __forceinline__ void f8_fragment(uint32_t w0, uint32_t w1, float sc, uint32_t (&a)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    uint32_t h2;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(static_cast<unsigned short>((i < 2 ? w0 : w1) >> (16 * (i & 1)))));
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h2));
+    a[i] = pack2_rn<T>(__fmul_rn(f.x, sc), __fmul_rn(f.y, sc));
+  }
+}
+
 __device__ __forceinline__ float ld_global_f32(const float* p) {
   float v;
   asm volatile("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
@@ -153,18 +168,24 @@ __device__ __forceinline__ float ld_global_f32(const float* p) {
 // Each thread reads its 16 nibble bytes of a k-block with one shared load and converts one k16 step at a time straight into the A
 // registers of a wgmma RS: step k + 1 is converted while step k's MMA runs (two fragment buffers, one commit group per step,
 // wgmma_wait<1>), so neither a shared-memory round trip nor a proxy fence sits on the MMA chain.
+// F8: the same register-A mainloop on e4m3 weights.  tmW streams the 8 KB tile (bytes permuted within the tile into fragment order,
+// so each thread reads a k-block's 32 bytes with two conflict-free 16-byte shared loads) and tmW2 the tile's 16 B of block scales;
+// warpgroup g's 64 rows share one scale per k-block.
 template <typename T, int MPAD, int EPI, bool XMC, int WQ>
 __global__ void __launch_bounds__(kGemmThreads, (MPAD >= 256 ? 1 : 2))
 skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmW2,
                   const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXh, const GemmParams p, const int stages,
                   const __grid_constant__ L2Prefetch pf) {
   constexpr bool kDual = (EPI == EPI_SWIGLU);
-  constexpr bool W8 = WQ == WQ_INT8, W4 = WQ == WQ_4BIT;
+  constexpr bool W8 = WQ == WQ_INT8, W4 = WQ == WQ_4BIT, F8 = WQ == WQ_FP8;
   static_assert(!XMC || (MPAD == 64 && !kDual), "X multicast: 64-row tiles, single accumulator");
   static_assert(WQ == WQ_NONE || (!XMC && !kDual), "W8A16 / W4A16: single weight stream, no X multicast");
-  constexpr int kWBytes = W8 ? kW8TileBytes : W4 ? kW4WBytes : kWTileBytes;  // weight bytes of one stage (per weight matrix)
-  constexpr int kStageBytes = W8 ? stage_bytes_w8(MPAD) : W4 ? stage_bytes_w4(MPAD) : stage_bytes(MPAD, EPI);
-  constexpr int kTxBytes = W4 ? kW4TileBytes + kW4AbsBytes + x_tile_bytes(MPAD) : kStageBytes;  // bytes TMA lands per stage
+  // weight bytes of one stage (per weight matrix)
+  constexpr int kWBytes = W8 ? kW8TileBytes : W4 ? kW4WBytes : F8 ? kF8WBytes : kWTileBytes;
+  constexpr int kStageBytes = W8 ? stage_bytes_w8(MPAD) : W4 ? stage_bytes_w4(MPAD) : F8 ? stage_bytes_fp8(MPAD) : stage_bytes(MPAD, EPI);
+  constexpr int kTxBytes = W4   ? kW4TileBytes + kW4AbsBytes + x_tile_bytes(MPAD)
+                           : F8 ? kF8TileBytes + kF8ScaleBytes + x_tile_bytes(MPAD)
+                                : kStageBytes;  // bytes TMA lands per stage
   constexpr int kPartBytes = acc_tile_bytes(MPAD, EPI);
 
   extern __shared__ uint8_t smem_raw[];
@@ -219,6 +240,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
         } else {
           tma_load_2d(st, &tmW, &full_bar[stage], kb * kBlockK, n_tile * kBlockN, kEvictFirst);
           if (kDual) tma_load_2d(st + kWTileBytes, &tmW2, &full_bar[stage], kb * kBlockK, n_tile * kBlockN, kEvictFirst);
+          if constexpr (F8) tma_load_2d(st + kF8TileBytes, &tmW2, &full_bar[stage], (kb / 2) * 4, n_tile, kEvictFirst);
         }
       };
       for (int j = 0; j < pre; ++j) load_w(j, kb_begin + j);
@@ -274,29 +296,44 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     }
     int s = 0, prev = -1;
     uint32_t ph = 0;
-    if constexpr (W4) {
-      pdl_wait();  // the code table is read with a generic load, which may not precede the dependency wait (X tiles follow it anyway)
-      if (threadIdx.x < 16)
-        asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_u32(w4_lut + threadIdx.x)), "f"(ld_global_f32(&kW4Codes[p.w4_quant][threadIdx.x]))
-                     : "memory");
-      asm volatile("bar.sync 2, 256;" ::: "memory");  // both MMA warpgroups see the table
-      // thread t of the warpgroup: its 16 bytes of every tile at (wg * 128 + t) * 16, word k = k16 step k; absmax of rows r0, r0 + 8
+    if constexpr (W4 || F8) {
+      if constexpr (W4) {
+        pdl_wait();  // the code table is read with a generic load, which may not precede the dependency wait (X tiles follow it anyway)
+        if (threadIdx.x < 16)
+          asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_u32(w4_lut + threadIdx.x)), "f"(ld_global_f32(&kW4Codes[p.w4_quant][threadIdx.x]))
+                       : "memory");
+        asm volatile("bar.sync 2, 256;" ::: "memory");  // both MMA warpgroups see the table
+      }
+      // W4: thread t of the warpgroup: its 16 bytes of every tile at (wg * 128 + t) * 16, word k = k16 step k; absmax of rows r0, r0 + 8.
+      // F8: its 32 bytes at (wg * 128 + t) * 16 (steps 0, 1) and 4096 + (wg * 128 + t) * 16 (steps 2, 3), two words per step; s0 is
+      // the scale of the warpgroup's 64-row group.
       const uint32_t lut = smem_u32(w4_lut);
       const int t = threadIdx.x & 127;
       const int r0 = wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
-      uint32_t q[4], a[2][4];
+      uint32_t q[F8 ? 8 : 4], a[2][4];
       float s0 = 0.f, s1 = 0.f;
       auto fetch = [&](int stage) {
         const uint32_t st = smem_u32(smem + stage * kStageBytes);
         asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]) : "r"(st + (threadIdx.x & 255) * 16)
                      : "memory");
-        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(s0) : "r"(st + kW4TileBytes + r0 * 4) : "memory");
-        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(s1) : "r"(st + kW4TileBytes + (r0 + 8) * 4) : "memory");
+        if constexpr (F8) {
+          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7])
+                       : "r"(st + kF8TileBytes / 2 + (threadIdx.x & 255) * 16)
+                       : "memory");
+          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(s0) : "r"(st + kF8TileBytes + wg * 4) : "memory");
+        } else {
+          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(s0) : "r"(st + kW4TileBytes + r0 * 4) : "memory");
+          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(s1) : "r"(st + kW4TileBytes + (r0 + 8) * 4) : "memory");
+        }
+      };
+      auto fragment = [&](int k, uint32_t(&frag)[4]) {  // k16 step k of the fetched k-block
+        if constexpr (F8) f8_fragment<T>(q[(k >> 1) * 4 + (k & 1) * 2], q[(k >> 1) * 4 + (k & 1) * 2 + 1], s0, frag);
+        else w4_fragment<T>(q[k], lut, s0, s1, frag);
       };
       if (kb_begin < kb_end) {
         mbar_wait_mma(&full_bar[0], 0);
         fetch(0);
-        w4_fragment<T>(q[0], lut, s0, s1, a[0]);
+        fragment(0, a[0]);
       }
       for (int kb = kb_begin; kb < kb_end; ++kb) {
         const uint64_t b_desc = make_kmajor_sw128_desc(smem_u32(smem + s * kStageBytes) + kWBytes);
@@ -308,12 +345,12 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
           wgmma_wait<1>();  // step k - 1 has retired: its fragment buffer a[(k + 1) & 1] may be rewritten
           if (k == 0 && prev >= 0) release(prev);  // ... and with it the previous k-block's last MMA
           if (k < 3) {
-            w4_fragment<T>(q[k + 1], lut, s0, s1, a[(k + 1) & 1]);
+            fragment(k + 1, a[(k + 1) & 1]);
           } else if (kb + 1 < kb_end) {
             const int sn = s + 1 == stages ? 0 : s + 1;
             mbar_wait_mma(&full_bar[sn], sn == 0 ? ph ^ 1 : ph);
             fetch(sn);
-            w4_fragment<T>(q[0], lut, s0, s1, a[0]);
+            fragment(0, a[0]);
           }
         }
         prev = s;
@@ -323,7 +360,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
         }
       }
     }
-    for (int kb = kb_begin; kb < kb_end && !W4; ++kb) {
+    for (int kb = kb_begin; kb < kb_end && !W4 && !F8; ++kb) {
       mbar_wait_mma(&full_bar[s], ph);
       const uint32_t st = smem_u32(smem + s * kStageBytes);
       uint32_t a_addr = st + wg * (kWTileBytes / 2);  // 64 weight rows = 8 KB = eight whole swizzle atoms
@@ -533,7 +570,10 @@ static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const C
   auto kern = skinny_gemm_wgmma<T, MPAD, EPI, XMC, WQ>;
   dim3 grid((p.N + kBlockN - 1) / kBlockN, p.splitk);
   const int stages = stage_count_for(MPAD, EPI, static_cast<int>(grid.x * grid.y), WQ);
-  const int sbytes = WQ == WQ_INT8 ? stage_bytes_w8(MPAD) : WQ == WQ_4BIT ? stage_bytes_w4(MPAD) : stage_bytes(MPAD, EPI);
+  const int sbytes = WQ == WQ_INT8   ? stage_bytes_w8(MPAD)
+                     : WQ == WQ_4BIT ? stage_bytes_w4(MPAD)
+                     : WQ == WQ_FP8  ? stage_bytes_fp8(MPAD)
+                                     : stage_bytes(MPAD, EPI);
   const int smem = stages * sbytes + (WQ == WQ_INT8 ? kW8DqBytes : 0) + kCtrlBytes + 1024;
   if (p.splitk > 8) return static_cast<int>(cudaErrorInvalidValue);  // portable cluster size
   // the accumulators are parked as (1|2) x MPAD x 128 fp32 partials (+ a 4 KB exchange strip) in the stage memory
@@ -599,7 +639,7 @@ int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUte
   return static_cast<int>(cudaErrorInvalidValue);
 }
 
-// W8A16 / W4A16: the epilogues of the target's decoder layer (+ EPI_STORE for mpad 16 / 64); w2: W4's absmax map
+// W8A16 / W4A16: the epilogues of the target's decoder layer (+ EPI_STORE for mpad 16 / 64); w2: W4's absmax map, FP8's scale map
 template <typename T, int MPAD, int WQ>
 static int launch_wq_epi(int epi, const CUtensorMap* w, const CUtensorMap* w2, const CUtensorMap* x, const GemmParams& p, cudaStream_t s,
                          const L2Prefetch* pf) {
@@ -645,6 +685,50 @@ int launch_gemm_w4(int dtype, int mpad, int epi, const CUtensorMap* tmW, const C
   if (p.splitk < 1 || p.m_rows > mpad || !tmA || p.K % kBlockK || (p.w4_quant != W4_NF4 && p.w4_quant != W4_FP4))
     return static_cast<int>(cudaErrorInvalidValue);
   return launch_wq<WQ_4BIT>(dtype, mpad, epi, tmW, tmA, tmX, p, s, pf);
+}
+
+int launch_gemm_fp8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmS, const CUtensorMap* tmX, const GemmParams& p_in,
+                    cudaStream_t s, const L2Prefetch* pf) {
+  GemmParams p = p_in;
+  if (p.splitk < 1 || p.m_rows > mpad || !tmS || p.K % 128 || p.N % kBlockN) return static_cast<int>(cudaErrorInvalidValue);
+  return launch_wq<WQ_FP8>(dtype, mpad, epi, tmW, tmS, tmX, p, s, pf);
+}
+
+// one thread per source byte and per source scale of a 64-row group; see kernels.h for the layouts
+__global__ void fp8_repack_kernel(const uint8_t* __restrict__ src, const float* __restrict__ src_scale, int nr, int K, int row0, int half,
+                                  uint8_t* __restrict__ dst, float* __restrict__ dst_scale, int n_rows) {
+  const int kc_n = K / 128;
+  const long n_bytes = src ? static_cast<long>(nr) * K : 0, n_sc = src_scale ? static_cast<long>(nr / 64) * kc_n : 0;
+  for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < n_bytes + n_sc; i += static_cast<long>(gridDim.x) * blockDim.x) {
+    if (i >= n_bytes) {
+      const int g = static_cast<int>((i - n_bytes) / kc_n), kc = static_cast<int>((i - n_bytes) % kc_n);  // 64-row group, 128-column block
+      const int d = half >= 0 ? g * 128 + half * 64 : row0 + g * 64;
+      if (d >= n_rows) continue;  // the launcher checks the destination; this keeps a bad call inside the buffers
+      dst_scale[(static_cast<long>(d / kBlockN) * kc_n + kc) * 4 + (d % kBlockN) / 64] = src_scale[static_cast<long>(g / 2) * kc_n + kc];
+      continue;
+    }
+    const int row = static_cast<int>(i / K), col = static_cast<int>(i % K);
+    const int d = half >= 0 ? (row / 64) * 128 + half * 64 + row % 64 : row0 + row;
+    if (d >= n_rows) continue;
+    // element (r, kk) of the 128 x 64 tile: k16 step kk / 16, column j of it; the thread and register that hold it in the A fragment
+    const int r = d % kBlockN, kk = col % kBlockK, step = kk / 16, j = kk % 16;
+    const int tidx = (r / 64) * 128 + ((r % 64) / 16) * 32 + (r % 8) * 4 + (j % 8) / 2;
+    const int reg = (j / 8) * 2 + (r % 16) / 8;
+    const int o = (step / 2) * (kF8TileBytes / 2) + tidx * 16 + (step % 2) * 8 + reg * 2 + (j & 1);  // byte offset in the stage
+    dst[static_cast<long>(d - r + o / kBlockK) * K + (col - kk) + o % kBlockK] = src[i];
+  }
+}
+int launch_fp8_repack(const uint8_t* src, const float* src_scale, int nr, int K, int row0, int half, uint8_t* dst, float* dst_scale,
+                      int n_rows, cudaStream_t s) {
+  if (nr < 0 || nr % 128 || K <= 0 || K % 128 || n_rows % kBlockN || (src && !dst) || (src_scale && !dst_scale))
+    return static_cast<int>(cudaErrorInvalidValue);
+  if (half >= 0 ? 2L * nr > n_rows : (row0 < 0 || row0 % 64 || static_cast<long>(row0) + nr > n_rows))
+    return static_cast<int>(cudaErrorInvalidValue);  // destination rows beyond the buffers
+  const long total = (src ? static_cast<long>(nr) * K : 0) + (src_scale ? static_cast<long>(nr / 64) * (K / 128) : 0);
+  if (total == 0) return 0;
+  const int blocks = static_cast<int>(std::min<long>((total + 255) / 256, 8192));
+  fp8_repack_kernel<<<blocks, 256, 0, s>>>(src, src_scale, nr, K, row0, half, dst, dst_scale, n_rows);
+  return static_cast<int>(cudaGetLastError());
 }
 
 // one thread per source byte (nibbles) and per source absmax; see kernels.h for the layouts

@@ -34,8 +34,15 @@ constexpr int kW4TileBytes = kBlockN * kBlockK / 2;
 constexpr int kW4AbsBytes = kBlockN * 4;
 constexpr int kW4WBytes = 5 * 1024;
 __host__ __device__ constexpr int stage_bytes_w4(int mpad) { return kW4WBytes + x_tile_bytes(mpad); }
+// W8A16 on FP8 (transformers' fine-grained e4m3, one fp32 scale per 128 x 128 block): a stage holds the 8 KB e4m3 tile, its bytes
+// permuted within the tile into fragment order (launch_fp8_repack), the tile's two 64-row-group scales of the k-block (16 B, two used),
+// padding to 1 KB so the X tile stays 1024-byte aligned, and the X tile
+constexpr int kF8TileBytes = kBlockN * kBlockK;
+constexpr int kF8ScaleBytes = 16;
+constexpr int kF8WBytes = 9 * 1024;
+__host__ __device__ constexpr int stage_bytes_fp8(int mpad) { return kF8WBytes + x_tile_bytes(mpad); }
 // weight modes of skinny_gemm_wgmma
-enum WeightQuant : int { WQ_NONE = 0, WQ_INT8 = 1, WQ_4BIT = 2 };
+enum WeightQuant : int { WQ_NONE = 0, WQ_INT8 = 1, WQ_4BIT = 2, WQ_FP8 = 3 };
 
 // number of SMs of the current device (the grids are sized to fill it)
 inline int device_sm_count() {

@@ -123,6 +123,20 @@ int launch_gemm_w4(int dtype, int mpad, int epi, const CUtensorMap* tmW, const C
 // A-fragment bytes contiguous (16 B); absmax lands transposed in [K / 64][n_pad].  K % 64 == 0.
 int launch_w4_repack(const uint8_t* src, const float* src_absmax, int nr, int K, int row0, int half, uint8_t* dst, float* dst_absmax,
                      int n_pad, cudaStream_t s);
+// W8A16 form on FP8 weights (transformers' FineGrainedFP8Config: e4m3, one fp32 weight_scale_inv per 128 x 128 block): tmW maps the
+// e4m3 [N][K] written by launch_fp8_repack exactly like an int8 weight (box 128 rows x 64 bytes, so the L2 prefetch plan applies
+// unchanged), tmS the block scales [N / 128][K / 128][4] fp32 (box 4 x 1).  The MMA warpgroups convert each k16 step into their
+// wgmma A fragments, W' = T(fp32(q) * scale) (one fp32 product, one round-to-nearest cast), while the previous step's MMA runs, so
+// the result is bit-identical to launch_gemm on W'.  N % 128 == 0, K % 128 == 0; epilogues and mpad as launch_gemm_w8.
+int launch_gemm_fp8(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmS, const CUtensorMap* tmX, const GemmParams& p,
+                    cudaStream_t s, const L2Prefetch* pf = nullptr);
+// Load-time repack of transformers' FP8 layout into the kernel's.  Source row i (of nr, a multiple of 128) of an e4m3 [nr][K] matrix
+// goes to destination row d(i) = row0 + i (row0 % 64 == 0), or, for half >= 0, to the gate/up interleave (i / 64) * 128 + half * 64 +
+// i % 64; within each 128 x 64 tile the bytes are permuted so that thread t of the MMA warpgroups finds its A-fragment bytes of k16
+// steps 0, 1 at 16 t and of steps 2, 3 at 4096 + 16 t.  The scales [nr / 128][K / 128] land per 64-row destination group: entry
+// (d / 64) % 2 of [n_rows / 128][K / 128][4] (entries 2, 3 stay as they are).  K % 128 == 0, n_rows % 128 == 0.
+int launch_fp8_repack(const uint8_t* src, const float* src_scale, int nr, int K, int row0, int half, uint8_t* dst, float* dst_scale,
+                      int n_rows, cudaStream_t s);
 // bring-up / debugging aid: same epilogues, plain FMA main loop, no TMA/wgmma.  W/W2/X are raw pointers.
 int launch_gemm_simt(int dtype, int mpad, int epi, const void* W, const void* W2, const void* X, long ldx,
                      const GemmParams& p, cudaStream_t s);

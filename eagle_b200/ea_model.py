@@ -20,11 +20,11 @@ from typing import Dict, Iterator, Optional
 import torch
 
 from . import _lib
-from .quant import is_target_projection, quantize_4bit, quantize_int8_rowwise
+from .quant import is_target_projection, quantize_4bit, quantize_fp8_block, quantize_int8_rowwise
 
 _TORCH2ENGINE = {torch.bfloat16: _lib.DT_BF16, torch.float16: _lib.DT_FP16, torch.float32: _lib.DT_FP32,
                  torch.int64: _lib.DT_INT64, torch.bool: _lib.DT_BOOL, torch.int8: _lib.DT_INT8,
-                 torch.uint8: _lib.DT_UINT8}
+                 torch.uint8: _lib.DT_UINT8, torch.float8_e4m3fn: _lib.DT_FP8_E4M3}
 
 
 def _llama3_inv_freq(inv_freq: torch.Tensor, rs: dict, max_position_embeddings: int) -> torch.Tensor:
@@ -157,21 +157,28 @@ class EaModel(torch.nn.Module):
         self.max_length = int(max_length)
         # int8 target projections (eagle_b200.quant): bitsandbytes' weight format, exact W8A16 arithmetic
         self.load_in_8bit = bool(load_in_8bit)
-        # quantization_config (a transformers BitsAndBytesConfig or its dict): load_in_4bit gives 4-bit target projections in
-        # bitsandbytes' nf4 / fp4 format with exact W4A16 arithmetic (eagle_b200.quant), load_in_8bit the int8 ones
-        from .checkpoint import quantization_config_dict, target_weights_4bit
+        # quantization_config (a transformers BitsAndBytesConfig / FineGrainedFP8Config or its dict): load_in_4bit gives 4-bit
+        # target projections in bitsandbytes' nf4 / fp4 format with exact W4A16 arithmetic (eagle_b200.quant), load_in_8bit the
+        # int8 ones, quant_method "fp8" transformers' fine-grained FP8 ones (128 x 128 block scales, exact W8A16 arithmetic)
+        from .checkpoint import quantization_config_dict, target_weights_4bit, target_weights_fp8
         qc = quantization_config_dict(quantization_config)
         self.quant_4bit = target_weights_4bit(qc, torch_dtype)
-        if qc and not self.quant_4bit:
+        self.quant_fp8 = target_weights_fp8(qc, target_config.get("num_hidden_layers", 1))
+        if qc and not self.quant_4bit and not self.quant_fp8:
             if not qc.get("load_in_8bit"):
-                raise ValueError("quantization_config: supported are bitsandbytes load_in_4bit (nf4 / fp4) and load_in_8bit")
+                raise ValueError("quantization_config: supported are bitsandbytes load_in_4bit (nf4 / fp4) and load_in_8bit, "
+                                 "and FineGrainedFP8Config (quant_method 'fp8')")
             self.load_in_8bit = True
         if self.quant_4bit and self.load_in_8bit:
             raise ValueError("load_in_8bit and a 4-bit quantization_config exclude each other")
+        if self.quant_fp8 and self.load_in_8bit:
+            raise ValueError("load_in_8bit and an FP8 quantization_config exclude each other")
         if self.load_in_8bit:
             flags |= _lib.FLAG_TARGET_INT8
         if self.quant_4bit:
             flags |= _lib.FLAG_TARGET_NF4 if self.quant_4bit == "nf4" else _lib.FLAG_TARGET_FP4
+        if self.quant_fp8:
+            flags |= _lib.FLAG_TARGET_FP8
         # attributes callers touch (ea_model.py:168; evaluation scripts)
         self.ea_layer = SimpleNamespace(total_tokens=total_token - 1, depth=depth, top_k=top_k)
         self.base_model = SimpleNamespace(config=self.config, dtype=torch_dtype, device=torch.device("cuda", int(device)))
@@ -221,7 +228,8 @@ class EaModel(torch.nn.Module):
     # weights
     # ---------------------------------------------------------------------------------------------
     def _load(self, name: str, t: torch.Tensor):
-        if t.dtype.is_floating_point and t.dtype != self.dtype and not name.endswith((".SCB", ".absmax")):
+        if t.dtype.is_floating_point and t.dtype != self.dtype and t.dtype != torch.float8_e4m3fn and \
+                not name.endswith((".SCB", ".absmax", ".weight_scale_inv")):
             t = t.to(self.dtype)  # `.to(base_model.dtype)` (ea_model.py:77)
         t = t.contiguous()
         if t.is_cuda:
@@ -231,8 +239,9 @@ class EaModel(torch.nn.Module):
         _lib.check(self.lib.eb200_load_tensor(self._h, name.encode(), t.data_ptr(), shape, t.dim(), _TORCH2ENGINE[t.dtype]))
 
     def _load_target(self, name: str, t: torch.Tensor):
-        """One target tensor; with load_in_8bit (4-bit) a model-dtype projection weight is quantized here (eagle_b200.quant), one
-        tensor at a time, and goes in as its int8 weight + SCB pair (uint8 codes + `.weight.absmax`)."""
+        """One target tensor; with load_in_8bit (4-bit, FP8) a model-dtype projection weight is quantized here (eagle_b200.quant),
+        one tensor at a time, on the tensor's device, and goes in as its int8 weight + SCB pair (uint8 codes + `.weight.absmax`;
+        float8_e4m3fn weight + `.weight_scale_inv`)."""
         if self.load_in_8bit and t.dtype.is_floating_point and name.endswith(".weight") and is_target_projection(name):
             q, scb = quantize_int8_rowwise(t.to(self.dtype))
             self._load(name, q)
@@ -241,6 +250,11 @@ class EaModel(torch.nn.Module):
             packed, absmax = quantize_4bit(t.to(self.dtype), self.quant_4bit)
             self._load(name, packed)
             self._load(name + ".absmax", absmax)
+        elif self.quant_fp8 and t.dtype.is_floating_point and t.dtype != torch.float8_e4m3fn and name.endswith(".weight") and \
+                is_target_projection(name):
+            q, scale_inv = quantize_fp8_block(t.to(self.dtype))
+            self._load(name, q)
+            self._load(name[: -len("weight")] + "weight_scale_inv", scale_inv)
         else:
             self._load(name, t)
 
@@ -309,10 +323,12 @@ class EaModel(torch.nn.Module):
         model.safetensors).  kwargs honoured: torch_dtype, max_length, device, tree_choices, load_in_8bit (int8 target projections,
         eagle_b200.quant; a checkpoint saved in transformers' bitsandbytes 8-bit format loads its int8 values as stored),
         quantization_config (a BitsAndBytesConfig or its dict: load_in_4bit with nf4 / fp4 gives 4-bit target projections; a
-        checkpoint saved in transformers' bitsandbytes 4-bit format loads its codes as stored); HF placement knobs (`device_map`,
-        `low_cpu_mem_usage`) are accepted with a warning, a bare load_in_4bit and anything else raise."""
-        from .checkpoint import (check_4bit_checkpoint, iter_4bit_triples, iter_checkpoint_tensors, iter_int8_pairs,
-                                 quantization_config_dict, read_json, target_weights_4bit, target_weights_int8)
+        checkpoint saved in transformers' bitsandbytes 4-bit format loads its codes as stored; a FineGrainedFP8Config or its dict
+        gives FP8 target projections, and a checkpoint saved in transformers' fine-grained FP8 format loads its FP8 weights as
+        stored); HF placement knobs (`device_map`, `low_cpu_mem_usage`) are accepted with a warning, a bare load_in_4bit and
+        anything else raise."""
+        from .checkpoint import (check_4bit_checkpoint, iter_4bit_triples, iter_checkpoint_tensors, iter_fp8_pairs, iter_int8_pairs,
+                                 quantization_config_dict, read_json, target_weights_4bit, target_weights_fp8, target_weights_int8)
         honoured = {"torch_dtype", "max_length", "device", "tree_choices", "load_in_8bit", "load_in_4bit", "quantization_config"}
         placement = {"device_map", "low_cpu_mem_usage"}  # HF / accelerate loading knobs
         unknown = set(kwargs) - honoured - placement
@@ -347,7 +363,19 @@ class EaModel(torch.nn.Module):
             raise ValueError(f"{base_model_path} is already quantized (quantization_config {tc['quantization_config']}); a 4-bit "
                              f"quantization_config applies to bf16 / fp16 checkpoints only")
         quant_4bit = stored_4bit or asked_4bit
-        int8 = False if quant_4bit else target_weights_int8(tc, kwargs.get("load_in_8bit", False) or bool(qc_arg.get("load_in_8bit")))
+        # FP8: a stored FP8 checkpoint is recognised only when no int8 request is made (load_in_8bit on it is refused by
+        # target_weights_int8, as before FP8 loaded); an FP8 quantization_config applies to bf16 / fp16 checkpoints or to a
+        # checkpoint already in that format
+        n_layers = tc.get("num_hidden_layers", 1)
+        asked_fp8 = target_weights_fp8(qc_arg, n_layers)
+        if asked_fp8 and asked_8bit:
+            raise ValueError("load_in_8bit and an FP8 quantization_config exclude each other")
+        stored_fp8 = not (quant_4bit or asked_8bit) and target_weights_fp8(tc.get("quantization_config"), n_layers)
+        if asked_fp8 and tc.get("quantization_config") and not stored_fp8:
+            raise ValueError(f"{base_model_path} is already quantized (quantization_config {tc['quantization_config']}); an FP8 "
+                             f"quantization_config applies to bf16 / fp16 checkpoints only")
+        fp8 = stored_fp8 or asked_fp8
+        int8 = False if (quant_4bit or fp8) else target_weights_int8(tc, kwargs.get("load_in_8bit", False) or bool(qc_arg.get("load_in_8bit")))
         hc = read_json(os.path.join(ea_model_path, "config.json"))
         tok = None
         try:
@@ -358,14 +386,16 @@ class EaModel(torch.nn.Module):
         m = cls(tc, hc, use_eagle3=use_eagle3, total_token=total_token, depth=depth, top_k=top_k, threshold=threshold,
                 torch_dtype=dtype, device=kwargs.get("device", 0), max_length=kwargs.get("max_length", 2048), tokenizer=tok,
                 tree_choices=kwargs.get("tree_choices"), load_in_8bit=int8,
-                quantization_config={"load_in_4bit": True, "bnb_4bit_quant_type": quant_4bit} if quant_4bit else None)
-        triples = iter_4bit_triples(base_model_path, stored_4bit, dtype) if stored_4bit else iter_int8_pairs(base_model_path)
+                quantization_config={"load_in_4bit": True, "bnb_4bit_quant_type": quant_4bit} if quant_4bit else
+                                    {"quant_method": "fp8"} if fp8 else None)
+        triples = iter_4bit_triples(base_model_path, stored_4bit, dtype) if stored_4bit else \
+            iter_fp8_pairs(base_model_path) if stored_fp8 else iter_int8_pairs(base_model_path)
         for k, v, aux in triples:
             if "rotary_emb" in k:
                 continue
-            if aux is not None:  # stored bitsandbytes int8 / 4-bit: loaded as is, not requantized
+            if aux is not None:  # stored bitsandbytes int8 / 4-bit / FP8: loaded as is, not requantized
                 m._load(k, v)
-                m._load(k + ".absmax" if stored_4bit else k[: -len("weight")] + "SCB", aux)
+                m._load(k + ".absmax" if stored_4bit else k[: -len("weight")] + ("weight_scale_inv" if stored_fp8 else "SCB"), aux)
             else:
                 m._load_target(k, v)
         head_sd = dict(iter_checkpoint_tensors(ea_model_path, prefer_bin=True))

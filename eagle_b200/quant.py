@@ -141,3 +141,52 @@ def decompress_nested_absmax(absmax_u8: torch.Tensor, nested_absmax: torch.Tenso
     scale = nested_absmax.float().repeat_interleave(int(nested_blocksize))[: a.numel()]
     out = nested_quant_map.float()[a] * scale
     return out + torch.tensor(float(nested_offset), dtype=torch.float32)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# FP8 target weights (`quantization_config=FineGrainedFP8Config()`, or a checkpoint with `quant_method: "fp8"`)
+#
+# transformers' fine-grained FP8 stores a [out, in] weight as `weight` float8_e4m3fn plus `weight_scale_inv` fp32
+# [out / 128, in / 128], one scale per 128 x 128 block.  The engine multiplies by
+#
+#     W' = dequantize_fp8_block(q, scale_inv, dtype) = dtype(fp32(q) * scale_inv[n // 128, k // 128])   (one product, one cast)
+#
+# which is transformers' own dequantization (Fp8Dequantize: `quantized.to(scales.dtype) * scales`, then the model-dtype cast),
+# so an FP8 engine computes bit for bit what a bf16 / fp16 engine loaded with W' computes.  FP8Linear's W8A8 arithmetic
+# (activations quantized per token group at run time, Triton / DeepGEMM kernels) is not reproduced: an FP8 engine's tokens are
+# those of W' in the model dtype.
+# ---------------------------------------------------------------------------------------------------------------------------
+FP8_BLOCK = 128
+FP8_MAX = 448.0  # torch.finfo(torch.float8_e4m3fn).max
+
+
+def quantize_fp8_block(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Blockwise FP8 quantization of a [out, in] weight (both multiples of 128) -> (q float8_e4m3fn [out, in], scale_inv fp32
+    [out / 128, in / 128]), restating transformers' Fp8Quantize.convert: per 128 x 128 block amax = max|fp32(w)|,
+    scale = 448 / amax (1 for an all-zero block), q = fp8(clamp(fp32(w) * scale, +-448)), scale_inv = fp32(1 / scale).
+    Runs on w's device."""
+    if w.dim() != 2 or not w.dtype.is_floating_point:
+        raise ValueError("quantize_fp8_block expects a floating-point [out, in] weight")
+    n, k = w.shape
+    if n % FP8_BLOCK or k % FP8_BLOCK:
+        raise ValueError(f"quantize_fp8_block: shape [{n}, {k}] is not a multiple of the {FP8_BLOCK} x {FP8_BLOCK} block")
+    q = torch.empty(n, k, dtype=torch.float8_e4m3fn, device=w.device)
+    scale_inv = torch.empty(n // FP8_BLOCK, k // FP8_BLOCK, dtype=torch.float32, device=w.device)
+    step = 8 * FP8_BLOCK  # rows per pass: the blocks are independent, and the fp32 temporaries of a 70B projection stay small
+    for r in range(0, n, step):
+        blocks = w[r: r + step].float().reshape(-1, FP8_BLOCK, k // FP8_BLOCK, FP8_BLOCK)
+        amax = blocks.abs().amax(dim=(1, 3))
+        scale = torch.where(amax > 0, FP8_MAX / torch.where(amax > 0, amax, torch.ones_like(amax)), torch.ones_like(amax))
+        q[r: r + step] = torch.clamp(blocks * scale[:, None, :, None], min=-FP8_MAX, max=FP8_MAX).to(torch.float8_e4m3fn).reshape(-1, k)
+        scale_inv[r // FP8_BLOCK: (r + step) // FP8_BLOCK] = (1.0 / scale).to(torch.float32)
+    return q, scale_inv
+
+
+def dequantize_fp8_block(q: torch.Tensor, scale_inv: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """W' = dtype(fp32(q) * scale_inv[n // 128, k // 128]): one fp32 product per element, then one round-to-nearest cast.  The
+    values the FP8 engine multiplies by."""
+    n, k = q.shape
+    s = scale_inv.float().repeat_interleave(FP8_BLOCK, dim=0).repeat_interleave(FP8_BLOCK, dim=1)
+    if s.shape != (n, k):
+        raise ValueError(f"dequantize_fp8_block: scale_inv {tuple(scale_inv.shape)} does not tile [{n}, {k}] in {FP8_BLOCK} x {FP8_BLOCK} blocks")
+    return (q.float() * s).to(dtype)

@@ -25,10 +25,11 @@
 extern "C" {
 #endif
 
-#define EB200_ABI_VERSION 3
+#define EB200_ABI_VERSION 4
 
 enum { EB200_BF16 = 0, EB200_FP16 = 1 };
-enum { EB200_DT_BF16 = 0, EB200_DT_FP16 = 1, EB200_DT_FP32 = 2, EB200_DT_INT64 = 3, EB200_DT_BOOL = 4, EB200_DT_INT8 = 5, EB200_DT_UINT8 = 6 };
+enum { EB200_DT_BF16 = 0, EB200_DT_FP16 = 1, EB200_DT_FP32 = 2, EB200_DT_INT64 = 3, EB200_DT_BOOL = 4, EB200_DT_INT8 = 5, EB200_DT_UINT8 = 6,
+       EB200_DT_FP8_E4M3 = 7 };
 
 typedef struct eb200_engine eb200_engine;
 
@@ -74,6 +75,12 @@ typedef struct eb200_config {
  * eb200_create already refuses them with tp_size > 1 (the loader places whole tensors). */
 #define EB200_FLAG_TARGET_NF4 16
 #define EB200_FLAG_TARGET_FP4 32
+/* The same projections stored the way transformers' FineGrainedFP8Config stores them: float8_e4m3fn weights with one fp32
+ * weight_scale_inv per 128 x 128 block, multiplied by a W8A16 GEMM that computes exactly what the model-dtype GEMM computes on
+ * W' = dtype(fp32(q) * weight_scale_inv[n / 128][k / 128]) (one fp32 product, one round-to-nearest cast).  Excludes the int8 and
+ * 4-bit flags; out- and in-features of every projection must be multiples of 128.  Same restrictions as int8, and eb200_create
+ * already refuses it with tp_size > 1 (the loader places whole tensors). */
+#define EB200_FLAG_TARGET_FP8 64
 
 typedef struct eb200_gen_params {
   float temperature, top_p;   /* eagenerate(temperature, top_p, top_k, ...) ea_model.py:199-208 */
@@ -106,7 +113,10 @@ void eb200_destroy(eb200_engine* e);
  * with); model-dtype data for those names is rejected, and so is int8 data anywhere else or for an engine without the flag.
  * EB200_FLAG_TARGET_NF4 / _FP4 engines take "model.layers.{i}.<proj>.weight" in EB200_DT_UINT8 [out, in / 2] (bitsandbytes' packing:
  * element 2j in the high nibble of byte j) plus "model.layers.{i}.<proj>.weight.absmax" in EB200_DT_FP32 [out, in / 64]; the engine
- * repacks both on the device into its kernel's private layout. */
+ * repacks both on the device into its kernel's private layout.
+ * EB200_FLAG_TARGET_FP8 engines take "model.layers.{i}.<proj>.weight" in EB200_DT_FP8_E4M3 [out, in] plus
+ * "model.layers.{i}.<proj>.weight_scale_inv" in EB200_DT_FP32 [out / 128, in / 128] (transformers' keys) and repack both on the
+ * device; model-dtype data for those names is rejected, and so is FP8 data anywhere else or for an engine without the flag. */
 int eb200_load_tensor(eb200_engine* e, const char* name, const void* data, const int64_t* shape, int32_t ndim,
                       int32_t dtype);
 /* cos/sin tables [n_pos][head_dim/2] in the model dtype, built by the caller exactly like the reference's
@@ -217,6 +227,11 @@ int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, const void*
                     const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
 /* the W4A16 GEMM (EB200_FLAG_TARGET_NF4 / _FP4) on bitsandbytes' layout: Wq uint8 [N, K/2], absmax fp32 [N, K/64], quant_type
  * 0 = nf4, 1 = fp4; the engine's load-time repack is applied first.  Epilogues and M as eb200_k_gemm_w8; K % 64 == 0. */
+/* the FP8 GEMM (EB200_FLAG_TARGET_FP8) on transformers' layout: Wq float8_e4m3fn [N, K], scale_inv fp32 [N/128, K/128]; the
+ * engine's load-time repack is applied first.  Epilogues and M as eb200_k_gemm_w8; K % 128 == 0 and the weight's rows (2N for the
+ * interleaved SwiGLU) a multiple of 128. */
+int eb200_k_gemm_fp8(int32_t dtype, int32_t epilogue, const void* Wq, const void* scale_inv, const void* X, void* out, const void* res,
+                     const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
 int eb200_k_gemm_w4(int32_t dtype, int32_t quant_type, int32_t epilogue, const void* Wq, const void* absmax, const void* X, void* out,
                     const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
 /* micro-benchmark of the skinny GEMM: `iters` back-to-back launches cycling over `n_weights` distinct [N,K] weight

@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""Int8 (load_in_8bit) or 4-bit (nf4 / fp4) target weights vs bf16 on bench.py's headline workload, in one process on one GPU.
+"""Int8 (load_in_8bit), 4-bit (nf4 / fp4) or FP8 (FineGrainedFP8Config) target weights vs bf16 on bench.py's headline workload, in one process on one GPU.
 
 Workload: Llama-3-8B shapes + EAGLE-3 head, bf16, 512-token prompt, 256 new tokens, greedy, dynamic tree (total_token=60,
 depth=6, top_k=10); random-init (default) or `--fixture correlated` weights, generated exactly like bench.py.  Two engines
 are built from the same weights: a quantized engine (the target's decoder projections as int8 + fp32 row scales, or with
-`--quant nf4|fp4` as bitsandbytes 4-bit codes + fp32 absmax per 64 weights) and a bf16 engine loaded with
+`--quant nf4|fp4` as bitsandbytes 4-bit codes + fp32 absmax per 64 weights, with `--quant fp8` as float8_e4m3fn + one fp32
+scale per 128 x 128 block) and a bf16 engine loaded with
 W' = dequantize(quantize(W)), the values the quantized engine multiplies by.  So the two must produce identical ids, which the
 run checks on the timed calls themselves.
 
@@ -12,14 +13,15 @@ Timing: after warm-up, `--rounds` rounds of one `--steps`-call window per engine
 window timed with CUDA events on the engine's stream (bench.timed_steps).  Prefill is timed separately (3 prefills).
 A separate profiled pass (per-launch CUDA events) gives the verify GEMMs' achieved bytes/s and their share of 3.35 TB/s.
 Bytes are algorithmic: every weight once per verify pass, the head once per draft pass (bench.weight_bytes_per_cycle);
-int8 projections count 1 byte per weight plus 4 bytes per row, 4-bit ones half a byte per weight plus 4 bytes per 64 weights.
+int8 projections count 1 byte per weight plus 4 bytes per row, 4-bit ones half a byte per weight plus 4 bytes per 64 weights,
+FP8 ones 1 byte per weight plus 16 bytes per 128 x 128 block (the kernel's padded scale layout).
 The card's name and power limit are read in the same run.
 
-`--model llama3-70b` (4-bit only: no bf16 twin fits on one card) builds one 4-bit engine with random weights, quantized per
+`--model llama3-70b` (4-bit or FP8: no bf16 twin fits on one card) builds one quantized engine with random weights, quantized per
 tensor on the device, and reports tok/s, tau, prefill, the engine's measured device footprint and how many generated tokens of
 greedy eagenerate equal naivegenerate's on the timed prompt.
 
-    python tools/w8_bench.py [--quant int8|nf4|fp4] [--model llama3-8b|llama3-70b] [--fixture random|correlated] [--rounds 3]
+    python tools/w8_bench.py [--quant int8|nf4|fp4|fp8] [--model llama3-8b|llama3-70b] [--fixture random|correlated] [--rounds 3]
                              [--steps 2] [--warmup 2] [--out FILE]
 """
 from __future__ import annotations
@@ -57,8 +59,10 @@ def card():
         return {"name": torch.cuda.get_device_name(0), "power_limit": None, "error": repr(ex)[:200]}
 
 
-def target_weights(args, tcfg, hcfg, dev):
-    """(name, tensor) of the target and the head, generated like bench.build_engine (random: streamed per tensor)."""
+def target_weights(args, tcfg, hcfg, dev, chunk_rows=None):
+    """(name, tensor) of the target and the head, generated like bench.build_engine (random: streamed per tensor).  chunk_rows:
+    draw random tensors that many rows at a time (other values than bench.py's, but no full-size fp32 temporary: a 70B FP8
+    engine leaves a few GB of the card free)."""
     dtype = torch.bfloat16
     if args.fixture == "correlated":
         _, tW, _, hW = syn.correlated_llama3_eagle3(tcfg["num_hidden_layers"], dtype, dev)
@@ -72,7 +76,12 @@ def target_weights(args, tcfg, hcfg, dev):
     gen = torch.Generator(device=dev)
     gen.manual_seed(0)
     for which, name, shape, kind in bench.weight_specs(tcfg, hcfg, True):
-        if kind == "normal":
+        if kind == "normal" and chunk_rows and len(shape) == 2:
+            w = torch.empty(shape, dtype=dtype, device=dev)
+            for r in range(0, shape[0], chunk_rows):
+                n = min(chunk_rows, shape[0] - r)
+                w[r: r + n] = (torch.randn((n, shape[1]), generator=gen, device=dev, dtype=torch.float32) * 0.02).to(dtype)
+        elif kind == "normal":
             w = (torch.randn(shape, generator=gen, device=dev, dtype=torch.float32) * 0.02).to(dtype)
         else:
             w = torch.ones(shape, dtype=dtype, device=dev) if kind == "ones" else torch.zeros(shape, dtype=dtype, device=dev)
@@ -82,6 +91,8 @@ def target_weights(args, tcfg, hcfg, dev):
 
 
 def quant_kwargs(q):
+    if q == "fp8":
+        return dict(quantization_config={"quant_method": "fp8", "activation_scheme": "dynamic", "weight_block_size": [128, 128]})
     return dict(load_in_8bit=True) if q == "int8" else dict(quantization_config={"load_in_4bit": True, "bnb_4bit_quant_type": q})
 
 
@@ -90,6 +101,9 @@ def quantize_pair(q, w):
     if q == "int8":
         qw, scb = quant.quantize_int8_rowwise(w)
         return [("weight", qw), ("SCB", scb)], quant.dequantize_int8_rowwise(qw, scb, torch.bfloat16)
+    if q == "fp8":
+        qw, scale_inv = quant.quantize_fp8_block(w)
+        return [("weight", qw), ("weight_scale_inv", scale_inv)], quant.dequantize_fp8_block(qw, scale_inv, torch.bfloat16)
     packed, absmax = quant.quantize_4bit(w, q)
     return [("weight", packed), ("weight.absmax", absmax)], quant.dequantize_4bit(packed, absmax, q, torch.bfloat16)
 
@@ -117,7 +131,7 @@ def build_pair(args):
 
 def bytes_per_cycle(tcfg, hcfg, q):
     """Algorithmic weight bytes of one cycle (bench.weight_bytes_per_cycle), with int8 projections at 1 B/weight + 4 B/row and
-    4-bit ones at 0.5 B/weight + 4 B per 64 weights (q: None for bf16)."""
+    4-bit ones at 0.5 B/weight + 4 B per 64 weights, FP8 ones at 1 B/weight + 16 B per 128 x 128 block (q: None for bf16)."""
     cyc, verify = bench.weight_bytes_per_cycle(tcfg, hcfg, True, bench.TREE["depth"])
     if not q:
         return cyc, verify
@@ -125,17 +139,18 @@ def bytes_per_cycle(tcfg, hcfg, q):
     for which, name, shape, kind in bench.weight_specs(tcfg, hcfg, True):
         if which == "t" and quant.is_target_projection(name):
             nk = shape[0] * shape[1]
-            saved += nk - 4 * shape[0] if q == "int8" else 2 * nk - (nk // 2 + 4 * (nk // 64))
+            saved += (nk - 4 * shape[0] if q == "int8" else nk - 16 * (nk // (128 * 128)) if q == "fp8"
+                      else 2 * nk - (nk // 2 + 4 * (nk // 64)))
     return cyc - saved, verify - saved
 
 
 def run_70b(args, info):
-    """One 4-bit Llama-3-70B + EAGLE-3 engine with random weights (quantized per tensor on the device)."""
+    """One 4-bit / FP8 Llama-3-70B + EAGLE-3 engine with random weights (quantized per tensor on the device)."""
     tcfg, hcfg, _ = bench.model_configs(argparse.Namespace(model="llama3-70b", layers=0))
     torch.cuda.synchronize()
     free0 = torch.cuda.mem_get_info()[0]
     m = EaModel(tcfg, hcfg, use_eagle3=True, torch_dtype=torch.bfloat16, device=0, max_length=2048, **quant_kwargs(args.quant), **bench.TREE)
-    for name, w in target_weights(args, tcfg, hcfg, "cuda:0"):
+    for name, w in target_weights(args, tcfg, hcfg, "cuda:0", chunk_rows=8192):
         if quant.is_target_projection(name):
             m._load_target(name, w)
         else:
@@ -193,7 +208,7 @@ def run_70b(args, info):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--quant", default="int8", choices=["int8", "nf4", "fp4"])
+    ap.add_argument("--quant", default="int8", choices=["int8", "nf4", "fp4", "fp8"])
     ap.add_argument("--model", default="llama3-8b", choices=["llama3-8b", "llama3-70b"])
     ap.add_argument("--fixture", default="random", choices=["random", "correlated"])
     ap.add_argument("--rounds", type=int, default=3)
@@ -204,7 +219,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("w8_bench.py: no CUDA device (eagle_b200 has no CPU path)")
     if args.model == "llama3-70b" and (args.quant == "int8" or args.fixture != "random"):
-        raise SystemExit("w8_bench.py: --model llama3-70b runs 4-bit (--quant nf4|fp4) random-init weights only")
+        raise SystemExit("w8_bench.py: --model llama3-70b runs 4-bit or FP8 (--quant nf4|fp4|fp8) random-init weights only")
     torch.cuda.set_device(0)
     info = card()
     log(f"card: {info}")
