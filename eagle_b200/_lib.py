@@ -114,6 +114,8 @@ SIGNATURES = {
     "eb200_k_sample_posterior": (_I32, [_I32, _P, _I32, _P, _P, _I32, _I32, _I32, C.c_float, C.c_float, _I32, _P, _I32,
                                          C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I32)]),
     "eb200_k_greedy_accept": (_I32, [_P, _P, _P, _I32, _I32, _I32, C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I32)]),
+    "eb200_k_sample_stats": (_I32, [_I32, _P, _I32, _I32, C.c_float, C.c_float, _I32, _P]),
+    "eb200_k_sample_token": (_I32, [_I32, _P, _I32, C.c_float, C.c_float, _I32, C.c_float, C.POINTER(_I32)]),
 }
 
 _lib = None

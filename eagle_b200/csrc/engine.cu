@@ -3631,3 +3631,59 @@ extern "C" int eb200_k_sample_posterior(int32_t dtype, const void* logits, int32
   if (uniforms_used) *uniforms_used = hst[S_UCOUNT];
   return 0;
 }
+
+// softmax statistics of the warped rows (row_softmax_stats_kernel): logits is a DEVICE [rows][V] model-dtype tensor,
+// stats (HOST) [rows][3] = max, sum, thr
+extern "C" int eb200_k_sample_stats(int32_t dtype, const void* logits, int32_t rows, int32_t V, float temperature, float top_p,
+                                    int32_t top_k, float* stats) {
+  if (dtype != EB200_BF16 && dtype != EB200_FP16) return fail("eb200_k_sample_stats: dtype must be bf16 or fp16");
+  if (!logits || !stats || rows < 1 || V < 1) return fail("eb200_k_sample_stats: bad arguments");
+  Scratch sc;
+  RowStats* d = sc.get<RowStats>(rows);
+  if (!d) return fail("scratch allocation failed");
+  SampleParams sp;
+  memset(&sp, 0, sizeof(sp));
+  sp.temperature = temperature;
+  sp.top_p = top_p;
+  sp.top_k = top_k;
+  CKL(launch_row_softmax_stats(dtype, logits, V, V, rows, sp, d, 0));
+  CK(cudaDeviceSynchronize());
+  std::vector<RowStats> h(rows);
+  CK(cudaMemcpy(h.data(), d, rows * sizeof(RowStats), cudaMemcpyDeviceToHost));
+  for (int r = 0; r < rows; ++r) {
+    stats[3 * r] = h[r].max;
+    stats[3 * r + 1] = h[r].sum;
+    stats[3 * r + 2] = h[r].thr;
+  }
+  return 0;
+}
+
+// one token drawn from logits row 0 exactly as sample_row0 draws the first token after prefill: the row's statistics, then
+// the inverse CDF (sample_commit_kernel, first_token = 1) with `u` as its uniform
+extern "C" int eb200_k_sample_token(int32_t dtype, const void* logits, int32_t V, float temperature, float top_p, int32_t top_k, float u,
+                                    int32_t* token) {
+  if (dtype != EB200_BF16 && dtype != EB200_FP16) return fail("eb200_k_sample_token: dtype must be bf16 or fp16");
+  if (!logits || !token || V < 1) return fail("eb200_k_sample_token: bad arguments");
+  Scratch sc;
+  TreeBuffers tb;
+  memset(&tb, 0, sizeof(tb));
+  RowStats* stats = sc.get<RowStats>(1);
+  int* st = sc.get<int>(S_COUNT);
+  float* un = sc.get<float>(1);
+  if (!un) return fail("scratch allocation failed");
+  CK(cudaMemcpy(un, &u, sizeof(float), cudaMemcpyHostToDevice));
+  SampleParams sp;
+  memset(&sp, 0, sizeof(sp));
+  sp.temperature = temperature;
+  sp.top_p = top_p;
+  sp.top_k = top_k;
+  sp.uniforms = un;
+  sp.n_uniforms = 1;
+  AcceptOut ao;
+  memset(&ao, 0, sizeof(ao));
+  CKL(launch_row_softmax_stats(dtype, logits, V, V, 1, sp, stats, 0));
+  CKL(launch_sample_commit(dtype, logits, V, V, stats, tb, 0, sp, nullptr, ao, st, nullptr, 0, 1, 0));
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(token, st + S_BONUS, sizeof(int), cudaMemcpyDeviceToHost));
+  return 0;
+}

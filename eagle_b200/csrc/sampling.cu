@@ -79,8 +79,10 @@ __global__ void __launch_bounds__(1024) row_softmax_stats_kernel(const T* __rest
   if (sp.top_p >= 1e-8f && sp.top_p < 1.0f) {
     // TopPLogitsWarper: ascending cumulative probability; tokens with cumulative mass <= 1 - top_p are removed.
     // Keep v iff mass(l <= l_v) > 1 - top_p  ->  bisect the smallest model-dtype value with that property (16 steps).
+    // The row maximum is always kept (min_tokens_to_keep = 1): the search ends at it even where no mass exceeds the cut,
+    // which happens when 1 - top_p rounds to 1 in fp32 (top_p below 2^-25).
     const float cut = (1.0f - sp.top_p) * z;
-    uint32_t lo = 0, hi = 0xffffu;  // keys; answer in [lo, hi]
+    uint32_t lo = 0, hi = order_key<T>(DT<T>::from_f(mx));  // keys; answer in [lo, hi]
     while (lo < hi) {
       const uint32_t mid = (lo + hi) >> 1;
       float m = 0.f;

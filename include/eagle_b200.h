@@ -312,6 +312,14 @@ int eb200_k_sample_posterior(int32_t dtype, const void* logits, int32_t V, const
                              int32_t T, int32_t n_leaf, int32_t max_depth, float temperature, float top_p, int32_t top_k,
                              const float* uniforms, int32_t n_uniforms, int32_t* best, int32_t* accept_length, int32_t* bonus,
                              int32_t* uniforms_used);
+/* softmax statistics of the warped rows (temperature -> top-p -> top-k) as the sampling posterior uses them: logits is a DEVICE
+ * [rows][V] model-dtype tensor; stats (HOST) [rows][3] = max, sum, thr, where p(v) = lt_v >= thr ? exp(lt_v - max) / sum : 0 */
+int eb200_k_sample_stats(int32_t dtype, const void* logits, int32_t rows, int32_t V, float temperature, float top_p, int32_t top_k,
+                         float* stats);
+/* one token drawn by inverse CDF from the warped logits row 0 (DEVICE [V], model dtype) with the uniform u: the draw of the
+ * first token after prefill and of vanilla sampling; token (HOST) */
+int eb200_k_sample_token(int32_t dtype, const void* logits, int32_t V, float temperature, float top_p, int32_t top_k, float u,
+                         int32_t* token);
 
 #ifdef __cplusplus
 }

@@ -482,31 +482,43 @@ def test_greedy_accept_matches_oracle(lib, seed):
 # ----------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("seed", range(8))
 @pytest.mark.parametrize("temperature,top_p,top_k", [(1.0, 0.0, 0), (0.7, 0.0, 0), (1.0, 0.9, 0), (1.3, 0.0, 20), (0.8, 0.95, 50)])
-def test_sample_posterior_matches_oracle(lib, seed, temperature, top_p, top_k):
+@pytest.mark.parametrize("V,dtype", [(512, torch.bfloat16), (32000, torch.float16), (128256, torch.bfloat16), (32003, torch.float16)],
+                         ids=["512-bf16", "32000-fp16", "128256-bf16", "32003-fp16"])
+def test_sample_posterior_matches_oracle(lib, V, dtype, seed, temperature, top_p, top_k):
+    """Decisions, uniforms drawn and the bonus token against tests/sampling_ref.posterior (the oracle's
+    evaluate_posterior_sampling on the rows as the stats kernel warped them; the thresholds of the rows the walk reads are
+    held to the float64 reference here, all of them by tests/test_sampling_gpu.py)."""
+    from tests import sampling_ref as sr
     g = torch.Generator().manual_seed(200 + seed)
-    k, depth, total, V = 10, 6, 60, 512
+    k, depth, total = 10, 6, 60
     scores, tokens, parents = _random_pool(k, depth, seed, torch.float32)
     scores = scores + torch.arange(scores.numel()) * 1e-7
     tokens = torch.randint(0, 40, (scores.numel(),), generator=g)  # small token range so candidates get real probability
     draft_tokens, retrieve, _, _ = orc.finalize_tree(scores, tokens, parents, torch.tensor([3]), k, total - 1, True)
-    logits_nodes = (torch.randn(total, V, generator=g) * 1.5).to(torch.bfloat16)
-    logits_nodes[:, :40] += 4.0  # the draft's token range is likely under the target too
-    uniforms = torch.rand(64, generator=g)
-    it = iter(uniforms.tolist())
-    # oracle in fp32 on the same (model-dtype-valued) logits; the engine keeps probabilities in fp32 too
-    warp = lambda lg: orc.warp_logits(lg, temperature, top_p, top_k)  # noqa: E731
-    lg32 = logits_nodes.float()
-    if temperature != 1.0:  # TemperatureLogitsWarper divides in the model dtype
-        lg32 = (logits_nodes / temperature).float()
-        warp = lambda lg: orc.warp_logits(lg, 1.0, top_p, top_k)  # noqa: E731
+    logits_nodes = (torch.randn(total, V, generator=g) * 1.5).to(dtype)
+    # the draft's token range is likely under the target too, about as likely at every vocabulary size
+    logits_nodes[:, :40] += 4.0 + math.log(V / 512)
+    lg_d = logits_nodes.cuda()
     cands = torch.cat((draft_tokens, torch.full((1, 1), -1, dtype=torch.long)), dim=1)[0, retrieve]
-    w_best, w_acc, w_p = orc.evaluate_posterior_sampling(lg32[retrieve], cands, warp, rand=lambda: next(it))
-    u_bonus = next(it)
-    cdf = torch.cumsum(w_p.double(), 0)
-    w_bonus = int(torch.searchsorted(cdf, torch.tensor(u_bonus * float(cdf[-1]), dtype=torch.float64)))
+    st = torch.zeros(total, 3)
+    check(lib, lib.eb200_k_sample_stats(DT[dtype], ptr(lg_d), total, V, temperature, top_p, top_k, ptr(st)))
+    thr = st[:, 2].double()
+    lt = sr.temperature_warp(logits_nodes, temperature)
+    for attempt in range(10):  # redraw uniforms that fall within rounding distance of an acceptance probability
+        uniforms = torch.rand(64, generator=g)
+        w_best, w_acc, w_p, w_used, ambiguous = sr.posterior(lt, thr, cands, retrieve, uniforms.tolist())
+        if not ambiguous:
+            break
+    assert not ambiguous
     best, acc, bonus, used = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int32()
-    check(lib, lib.eb200_k_sample_posterior(0, ptr(logits_nodes.cuda()), V, ptr(draft_tokens[0].int().contiguous()),
+    check(lib, lib.eb200_k_sample_posterior(DT[dtype], ptr(lg_d), V, ptr(draft_tokens[0].int().contiguous()),
                                             ptr(retrieve.int().contiguous()), total, retrieve.shape[0], retrieve.shape[1], temperature, top_p,
                                             top_k, ptr(uniforms.contiguous()), 64, C.byref(best), C.byref(acc), C.byref(bonus), C.byref(used)))
-    assert (best.value, acc.value) == (int(w_best), int(w_acc))
-    assert bonus.value == w_bonus or abs(float(cdf[bonus.value]) - u_bonus * float(cdf[-1])) < 1e-4
+    assert (best.value, acc.value) == (w_best, w_acc)
+    assert used.value == w_used
+    for node in retrieve[w_best, :w_acc + 1].tolist():  # the rows the walk and the bonus draw read
+        adm = sr.RowRef(lt[node]).admissible(top_p, top_k)
+        assert float(thr[node]) in adm, (node, float(thr[node]), sorted(adm)[:4])
+    ok = sr.bracket(w_p, float(uniforms[used.value - 1]), sr.cdf_delta_rel(V))
+    assert bool(ok[bonus.value]), (f"bonus {bonus.value} (p = {float(w_p[bonus.value]):.3g}) outside the bracket "
+                                   f"{torch.nonzero(ok).flatten()[:8].tolist()}")
