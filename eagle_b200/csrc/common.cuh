@@ -149,17 +149,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// same, delivered to the same shared-memory offset (and signalling the mbarrier at the same offset) of every CTA in cta_mask
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint16_t cta_mask,
-                                                      uint64_t cache_hint) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5, %6;"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask), "l"(cache_hint)
-      : "memory");
-}
-
 // ------------------------------------------------------------------------------------------
 // wgmma (Hopper warpgroup MMA): D[64 x N] (fp32, registers of the 128 threads of one warpgroup) += A[64 x 16] * B[N x 16]^T,
 // A and B read from shared memory through matrix descriptors, both K-major.
@@ -375,10 +364,6 @@ __device__ __forceinline__ float dsmem_ld_f32(uint32_t cluster_addr) {
   float v;
   asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(cluster_addr) : "memory");
   return v;
-}
-// arrive on the mbarrier at the offset of `bar` in the CTA of rank `rank` of this cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(dsmem_map(smem_u32(bar), rank)) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------

@@ -151,7 +151,7 @@ struct Linear {
 struct ActBuf {  // an activation buffer usable as the X operand of the GEMM (64 rows; 256 where the prompt prefill runs through it)
   void* p = nullptr;
   int cols = 0, rows = 64;
-  CUtensorMap tm16, tm32, tm64, tm256;  // tm32: half of a 64-row X tile (TMA multicast between neighbouring n-tiles)
+  CUtensorMap tm16, tm64, tm256;
 };
 struct Layer {
   Linear qkv, o, gu, down;  // gu: gate_proj and up_proj interleaved in 64-row groups (EPI_SWIGLU_IL)
@@ -224,7 +224,6 @@ struct eb200_engine {
   float* ws = nullptr;
   size_t ws_bytes = 0;
   size_t l2_bytes = 0;  // device L2 size: caps the weight bytes prefetched ahead of a GEMM
-  float* sk_ws = nullptr;  // stream-K partial slots
   int* counters = nullptr;
   // tree + cycle state
   int* st = nullptr;
@@ -338,7 +337,6 @@ static int alloc_act(eb200_engine* e, ActBuf& a, int cols, int rows = 64) {
   TRY(dalloc(e, &a.p, static_cast<size_t>(rows) * cols * 2));
   TRY(make_tmap(&a.tm16, e->dtype, a.p, rows, cols, 16));
   TRY(make_tmap(&a.tm64, e->dtype, a.p, rows, cols, 64));
-  TRY(make_tmap(&a.tm32, e->dtype, a.p, rows, cols, 32));
   if (rows >= 256) TRY(make_tmap(&a.tm256, e->dtype, a.p, rows, cols, 256));
   return 0;
 }
@@ -505,7 +503,6 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
       e->xn.cols = H;
       TRY(make_tmap(&e->xn.tm16, e->dtype, e->xn.p, 64, H, 16));
       TRY(make_tmap(&e->xn.tm64, e->dtype, e->xn.p, 64, H, 64));
-      TRY(make_tmap(&e->xn.tm32, e->dtype, e->xn.p, 64, H, 32));
       TRY(dalloc(e, reinterpret_cast<void**>(&e->tp_epoch), 64));
       TRY(dalloc(e, reinterpret_cast<void**>(&e->tp_ready_base), 64));
     } else {
@@ -533,7 +530,6 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
     e->ws_bytes = static_cast<size_t>(96) << 20;
     TRY(dalloc(e, reinterpret_cast<void**>(&e->ws), e->ws_bytes, false));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->counters), 8192 * sizeof(int)));
-    TRY(dalloc(e, reinterpret_cast<void**>(&e->sk_ws), streamk_ws_bytes(), false));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->chain_sync), 16 * sizeof(int)));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->chain_timing), 4 * sizeof(unsigned long long)));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->tile_val), static_cast<size_t>((e->V_l + 127) / 128) * 64 * sizeof(float)));
@@ -1015,7 +1011,6 @@ static int finalize_linear(eb200_engine* e, Linear& l, const char* what, uint64_
   return make_tmap(&l.tm, e->dtype, l.w, l.N, l.K, 128);
 }
 
-static int gemm_mode();
 extern "C" int eb200_finalize(eb200_engine* e) {
   if (!e) return fail("eb200_finalize: null engine");
   CK(cudaSetDevice(e->c.device));
@@ -1029,7 +1024,6 @@ extern "C" int eb200_finalize(eb200_engine* e) {
     if (e->c.tp_size > 1) what = "tensor parallelism (tp_size > 1)";
     else if (e->c.flags & EB200_FLAG_SIMT_GEMM) what = "EB200_FLAG_SIMT_GEMM";
     else if (chain && atoi(chain) == 1) what = "EB200_CHAIN=1 (persistent layer-segment launches)";
-    else if (gemm_mode() == 0) what = "EB200_GEMM_MODE=streamk";
     if (what)
       return fail("%s are not supported with %s; they run on one GPU with the default cluster split-K GEMM", fmt, what);
   }
@@ -1203,16 +1197,6 @@ static int pick_splitk(int N, int K, int mpad, int epi, size_t ws_bytes) {
   return std::min(sk, 8);
 }
 
-// 0 = persistent stream-K, 1 = cluster split-K (default)
-static int gemm_mode() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("EB200_GEMM_MODE");
-    v = (e && !strcmp(e, "streamk")) ? 0 : 1;  // cluster split-K is the faster one on the benchmark shapes (DESIGN.md)
-  }
-  return v;
-}
-
 // EB200_L2_PREFETCH=1 turns the L2 weight prefetch on; read once.  Off by default: on the H100 every window measured slower with
 // it (DESIGN.md §5), so it stays an experiment.
 static bool l2_prefetch_on() {
@@ -1306,14 +1290,10 @@ static int run_gemm(eb200_engine* e, const RowCtx& cx, GemmCall& g) {
     const size_t per_split = static_cast<size_t>(g.epi == EPI_SWIGLU ? 2 : 1) * cx.mpad * ((p.N + 127) / 128) * 128 * 4;
     while (p.splitk > 1 && per_split * p.splitk > e->ws_bytes) --p.splitk;
     CKL(launch_gemm_simt(e->dtype, cx.mpad, g.epi, g.W->w, g.W2 ? g.W2->w : nullptr, g.X->p, g.X->cols, p, e->stream));
-  } else if (gemm_mode() == 1) {
+  } else {
     if (cx.mpad == 256 && g.X->rows < 256) return fail("256-row GEMM on a 64-row activation buffer");
     CKL(launch_gemm(e->dtype, cx.mpad, g.epi, &g.W->tm, g.W2 ? &g.W2->tm : nullptr,
-                    cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256), p, e->stream, cx.mpad == 64 ? &g.X->tm32 : nullptr,
-                    g.pf));
-  } else {
-    CKL(launch_gemm_streamk(e->dtype, cx.mpad, g.epi, &g.W->tm, g.W2 ? &g.W2->tm : nullptr, cx.mpad == 16 ? &g.X->tm16 : &g.X->tm64, p,
-                            e->sk_ws, e->counters, e->stream));
+                    cx.mpad == 16 ? &g.X->tm16 : (cx.mpad == 64 ? &g.X->tm64 : &g.X->tm256), p, e->stream, g.pf));
   }
   return 0;
 }
@@ -2889,17 +2869,8 @@ extern "C" int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const
     TRY(make_tmap(&tw, dtype, W, N, K, 128));
     if (W2) TRY(make_tmap(&tw2, dtype, W2, N, K, 128));
     TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
-    CUtensorMap txh;
-    TRY(make_tmap(&txh, dtype, X, 64, K, 32));
-    const bool cluster = simt == 2 || (simt == 0 && gemm_mode() == 1);
-    if (cluster) {
-      if (p.splitk > 8) p.splitk = 8;
-      CKL(launch_gemm(dtype, mpad, epilogue, &tw, W2 ? &tw2 : nullptr, &tx, p, s, mpad == 64 ? &txh : nullptr));
-    } else {
-      float* skws = sc.get<float>(streamk_ws_bytes() / 4, false);
-      if (!skws) return fail("scratch allocation failed");
-      CKL(launch_gemm_streamk(dtype, mpad, epilogue, &tw, W2 ? &tw2 : nullptr, &tx, p, skws, counters, s));
-    }
+    if (p.splitk > 8) p.splitk = 8;
+    CKL(launch_gemm(dtype, mpad, epilogue, &tw, W2 ? &tw2 : nullptr, &tx, p, s));
   }
   CK(cudaStreamSynchronize(s));
   return 0;
@@ -2938,7 +2909,7 @@ extern "C" int eb200_k_prefetch(int32_t dtype, int32_t kernel, int32_t epilogue,
     CUtensorMap tw, tx;
     TRY(make_tmap(&tw, dtype, W, N, K, 128));
     TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
-    CKL(launch_gemm(dtype, mpad, epilogue, &tw, nullptr, &tx, p, s, nullptr, &pf));
+    CKL(launch_gemm(dtype, mpad, epilogue, &tw, nullptr, &tx, p, s, &pf));
   }
   CK(cudaStreamSynchronize(s));
   return 0;
@@ -3191,9 +3162,8 @@ extern "C" int eb200_k_gemm_bench(int32_t dtype, int32_t epilogue, int32_t M, in
   void* out = sc.get<uint16_t>(static_cast<size_t>(64) * N, true);
   if (!X || !out) return fail("allocation failed");
   (void)n_out;
-  CUtensorMap tx, txh;
+  CUtensorMap tx;
   TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
-  TRY(make_tmap(&txh, dtype, X, 64, K, 32));
   GemmParams p;
   memset(&p, 0, sizeof(p));
   p.N = N;
@@ -3205,16 +3175,12 @@ extern "C" int eb200_k_gemm_bench(int32_t dtype, int32_t epilogue, int32_t M, in
   p.ld_out = N;
   p.res = out;
   p.ld_res = N;
-  float* bws = sc.get<float>(streamk_ws_bytes() / 4, false);
-  int* bflags = sc.get<int>(8192);
-  if (!bws || !bflags) return fail("allocation failed");
   cudaStream_t s;
   CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
   auto run_all = [&]() -> int {
     for (int i = 0; i < iters; ++i) {
       const int wi = i % n_weights;
-      if (gemm_mode() == 1) CKL(launch_gemm(dtype, mpad, epilogue, &tw[wi], epilogue == EPI_SWIGLU ? &tw2[wi] : nullptr, &tx, p, s, mpad == 64 ? &txh : nullptr));
-      else CKL(launch_gemm_streamk(dtype, mpad, epilogue, &tw[wi], epilogue == EPI_SWIGLU ? &tw2[wi] : nullptr, &tx, p, bws, bflags, s));
+      CKL(launch_gemm(dtype, mpad, epilogue, &tw[wi], epilogue == EPI_SWIGLU ? &tw2[wi] : nullptr, &tx, p, s));
     }
     return 0;
   };
@@ -3290,17 +3256,8 @@ extern "C" int eb200_k_qkv_rope(int32_t dtype, int32_t simt, const void* Wqkv, c
     CUtensorMap tw, tx;
     TRY(make_tmap(&tw, dtype, Wqkv, N, K, 128));
     TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
-    CUtensorMap txh;
-    TRY(make_tmap(&txh, dtype, X, 64, K, 32));
-    const bool cluster = simt == 2 || (simt == 0 && gemm_mode() == 1);
-    if (cluster) {
-      if (p.splitk > 8) p.splitk = 8;
-      CKL(launch_gemm(dtype, mpad, EPI_QKV_ROPE, &tw, nullptr, &tx, p, s, mpad == 64 ? &txh : nullptr));
-    } else {
-      float* skws = sc.get<float>(streamk_ws_bytes() / 4, false);
-      if (!skws) return fail("scratch allocation failed");
-      CKL(launch_gemm_streamk(dtype, mpad, EPI_QKV_ROPE, &tw, nullptr, &tx, p, skws, counters, s));
-    }
+    if (p.splitk > 8) p.splitk = 8;
+    CKL(launch_gemm(dtype, mpad, EPI_QKV_ROPE, &tw, nullptr, &tx, p, s));
   }
   CK(cudaStreamSynchronize(s));
   return 0;

@@ -157,9 +157,6 @@ __device__ __forceinline__ float ld_global_f32(const float* p) {
 // (wgmma m64 x MPAD x k16, fp32 accumulators in registers); warp 8 is the TMA producer.  After the main loop both
 // warpgroups park their accumulators in the (then idle) stage memory as an fp32 [acc][MPAD][128] tile, and warpgroup 0
 // runs the epilogue from there (thread <-> weight row).
-// XMC: the two CTAs of neighbouring n-tiles (cluster dimension x = 2) stream the SAME activation k-range; each loads one half of
-// every X tile (32 rows) and TMA-multicasts it into both CTAs' rings, so the L2 -> shared-memory ingress of an SM carries half
-// the X bytes.
 // W8: tmW streams int8 weight tiles; the MMA warpgroups dequantize every stage into one model-dtype tile (an 8 KB half per
 // warpgroup) and run the same k16 MMAs on it, so the accumulators equal those of the kernel on the dequantized W.  Each k-block's
 // MMAs retire before the next dequantization (wgmma_wait<0>): ptxas serialises every wgmma of a kernel whose MMAs stay in flight
@@ -171,15 +168,13 @@ __device__ __forceinline__ float ld_global_f32(const float* p) {
 // F8: the same register-A mainloop on e4m3 weights.  tmW streams the 8 KB tile (bytes permuted within the tile into fragment order,
 // so each thread reads a k-block's 32 bytes with two conflict-free 16-byte shared loads) and tmW2 the tile's 16 B of block scales;
 // warpgroup g's 64 rows share one scale per k-block.
-template <typename T, int MPAD, int EPI, bool XMC, int WQ>
+template <typename T, int MPAD, int EPI, int WQ>
 __global__ void __launch_bounds__(kGemmThreads, (MPAD >= 256 ? 1 : 2))
 skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmW2,
-                  const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXh, const GemmParams p, const int stages,
-                  const __grid_constant__ L2Prefetch pf) {
+                  const __grid_constant__ CUtensorMap tmX, const GemmParams p, const int stages, const __grid_constant__ L2Prefetch pf) {
   constexpr bool kDual = (EPI == EPI_SWIGLU);
   constexpr bool W8 = WQ == WQ_INT8, W4 = WQ == WQ_4BIT, F8 = WQ == WQ_FP8;
-  static_assert(!XMC || (MPAD == 64 && !kDual), "X multicast: 64-row tiles, single accumulator");
-  static_assert(WQ == WQ_NONE || (!XMC && !kDual), "W8A16 / W4A16: single weight stream, no X multicast");
+  static_assert(WQ == WQ_NONE || !kDual, "W8A16 / W4A16: single weight stream");
   // weight bytes of one stage (per weight matrix)
   constexpr int kWBytes = W8 ? kW8TileBytes : W4 ? kW4WBytes : F8 ? kF8WBytes : kWTileBytes;
   constexpr int kStageBytes = W8 ? stage_bytes_w8(MPAD) : W4 ? stage_bytes_w4(MPAD) : F8 ? stage_bytes_fp8(MPAD) : stage_bytes(MPAD, EPI);
@@ -204,24 +199,20 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
   const int kb_begin = static_cast<int>((static_cast<long>(num_kb) * split) / p.splitk);
   const int kb_end = static_cast<int>((static_cast<long>(num_kb) * (split + 1)) / p.splitk);
   pdl_launch_dependents();  // let the next kernel start its own (independent) prologue and weight prefetch
-  // cluster = (XMC ? 2 : 1) x splitk x 1; rank = x + 2 * y when XMC
-  const uint32_t crank = (XMC || p.splitk > 1) ? cluster_ctarank() : 0u;
-  const uint32_t xpar = XMC ? (crank & 1u) : 0u;
-  const uint16_t pair_mask = XMC ? static_cast<uint16_t>(3u << (crank & ~1u)) : static_cast<uint16_t>(0);
+  // cluster = 1 x splitk x 1: the rank is this CTA's index among the split-K peers of its n-tile
+  const uint32_t crank = p.splitk > 1 ? cluster_ctarank() : 0u;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmW);
-    tma_prefetch_desc(XMC ? &tmXh : &tmX);
+    tma_prefetch_desc(&tmX);
     if (kDual) tma_prefetch_desc(&tmW2);
     for (int i = 0; i < stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      // one arrival per MMA warpgroup; XMC: also the neighbour's (its half of the X tile lives here too)
-      mbar_init(&empty_bar[i], XMC ? 4 : 2);
+      mbar_init(&empty_bar[i], 2);  // one arrival per MMA warpgroup
     }
     fence_barrier_init();
   }
-  if (XMC) cluster_sync_all();  // the neighbour's barriers exist before anything is multicast into this CTA
-  else __syncthreads();
+  __syncthreads();
 
   if (warp == kTmaWarp) {
     // ===== TMA producer =====
@@ -246,13 +237,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
       for (int j = 0; j < pre; ++j) load_w(j, kb_begin + j);
       pdl_wait();
       auto load_x = [&](int stage, int kb) {
-        uint8_t* xdst = smem + stage * kStageBytes + kWBytes * (kDual ? 2 : 1);
-        if constexpr (XMC) {
-          tma_load_2d_multicast(xdst + xpar * (32 * kBlockK * 2), &tmXh, &full_bar[stage], kb * kBlockK, static_cast<int>(xpar) * 32, pair_mask,
-                                kEvictLast);
-        } else {
-          tma_load_2d(xdst, &tmX, &full_bar[stage], kb * kBlockK, 0, kEvictLast);
-        }
+        tma_load_2d(smem + stage * kStageBytes + kWBytes * (kDual ? 2 : 1), &tmX, &full_bar[stage], kb * kBlockK, 0, kEvictLast);
       };
       for (int j = 0; j < pre; ++j) load_x(j, kb_begin + j);
       int s = (pre == stages) ? 0 : pre;
@@ -279,10 +264,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
 #pragma unroll
     for (int i = 0; i < (kDual ? MPAD / 2 : 1); ++i) acc2[i] = 0.f;
     auto release = [&](int st) {
-      if ((threadIdx.x & 127) == 0) {
-        mbar_arrive(&empty_bar[st]);
-        if constexpr (XMC) mbar_arrive_cluster(&empty_bar[st], crank ^ 1u);  // the neighbour's half of this slot is consumed too
-      }
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[st]);
     };
     float sc[2] = {0.f, 0.f};
     if constexpr (W8) {
@@ -422,7 +404,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
       const int row = threadIdx.x;
       const int m_valid = valid_rows(p);
       const int S = p.splitk;
-      const int rank = static_cast<int>(XMC ? (crank >> 1) : crank);  // this CTA's index among the split-K peers of its n-tile
+      const int rank = static_cast<int>(crank);
       const int per = (MPAD + S - 1) / S;  // activation rows reduced by each CTA
       const int m_lo = rank * per, m_hi = min(MPAD, m_lo + per);
       const uint32_t part_local = smem_u32(smem);
@@ -434,7 +416,7 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
 #pragma unroll
         for (int j = 0; j < 16; ++j) acc[j] = acc2[j] = 0.f;
         for (int s = 0; s < S; ++s) {  // fixed rank order: deterministic sums
-          const uint32_t peer = dsmem_map(part_local, XMC ? (xpar + 2u * static_cast<uint32_t>(s)) : static_cast<uint32_t>(s));
+          const uint32_t peer = dsmem_map(part_local, static_cast<uint32_t>(s));
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             if (j < nrows && m0 + j < m_valid) {
@@ -447,8 +429,6 @@ skinny_gemm_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant
       }
     }
     cluster_sync_all();  // no CTA may exit (and free its shared memory) while a peer still reads it
-  } else if (XMC) {
-    cluster_sync_all();  // the neighbour may still multicast into / arrive on this CTA's shared memory
   }
 }
 
@@ -542,32 +522,10 @@ const void* silu_lut(int dtype, cudaStream_t s) {
 // ------------------------------------------------------------------------------------------------------------
 // host launchers
 // ------------------------------------------------------------------------------------------------------------
-static bool xmc_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    // Opt-in: correct (all GEMM parity tests pass with it), but it doubles the cluster size of the split-K projections, which
-    // constrains their scheduling, and has no measured gain on the H100.
-    const char* e = getenv("EB200_GEMM_XMC");
-    v = (e && atoi(e) == 1) ? 1 : 0;
-  }
-  return v == 1;
-}
-template <typename T, int MPAD, int EPI, bool XMC, int WQ = WQ_NONE>
-static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
-                        cudaStream_t s, const L2Prefetch* pf);
-template <typename T, int MPAD, int EPI>
+template <typename T, int MPAD, int EPI, int WQ = WQ_NONE>
 static int launch_one(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const GemmParams& p, cudaStream_t s,
-                      const CUtensorMap* tmXh, const L2Prefetch* pf) {
-  if constexpr (MPAD == 64 && EPI != EPI_SWIGLU) {
-    const int tiles = (p.N + kBlockN - 1) / kBlockN;
-    if (tmXh && xmc_enabled() && tiles % 2 == 0 && 2 * p.splitk <= 8) return launch_one_x<T, MPAD, EPI, true>(tmW, tmW2, tmX, tmXh, p, s, pf);
-  }
-  return launch_one_x<T, MPAD, EPI, false>(tmW, tmW2, tmX, tmX, p, s, pf);
-}
-template <typename T, int MPAD, int EPI, bool XMC, int WQ>
-static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX, const CUtensorMap* tmXh, const GemmParams& p,
-                        cudaStream_t s, const L2Prefetch* pf) {
-  auto kern = skinny_gemm_wgmma<T, MPAD, EPI, XMC, WQ>;
+                      const L2Prefetch* pf) {
+  auto kern = skinny_gemm_wgmma<T, MPAD, EPI, WQ>;
   dim3 grid((p.N + kBlockN - 1) / kBlockN, p.splitk);
   const int stages = stage_count_for(MPAD, EPI, static_cast<int>(grid.x * grid.y), WQ);
   const int sbytes = WQ == WQ_INT8   ? stage_bytes_w8(MPAD)
@@ -589,20 +547,20 @@ static int launch_one_x(const CUtensorMap* tmW, const CUtensorMap* tmW2, const C
   }
   L2Prefetch none;
   memset(&none, 0, sizeof(none));
-  return static_cast<int>(launch_kc(kern, grid, dim3(kGemmThreads), static_cast<size_t>(smem), s, dim3(XMC ? 2 : 1, p.splitk, 1), *tmW,
-                                    tmW2 ? *tmW2 : *tmW, *tmX, *tmXh, p, stages, pf ? *pf : none));
+  return static_cast<int>(launch_kc(kern, grid, dim3(kGemmThreads), static_cast<size_t>(smem), s, dim3(1, p.splitk, 1), *tmW,
+                                    tmW2 ? *tmW2 : *tmW, *tmX, p, stages, pf ? *pf : none));
 }
 
 template <typename T, int MPAD>
 static int launch_epi(int epi, const CUtensorMap* a, const CUtensorMap* b, const CUtensorMap* c, const GemmParams& p,
-                      cudaStream_t s, const CUtensorMap* ch, const L2Prefetch* pf) {
+                      cudaStream_t s, const L2Prefetch* pf) {
   switch (epi) {
-    case EPI_STORE: return launch_one<T, MPAD, EPI_STORE>(a, b, c, p, s, ch, pf);
-    case EPI_RESIDUAL: return launch_one<T, MPAD, EPI_RESIDUAL>(a, b, c, p, s, ch, pf);
-    case EPI_SWIGLU: return launch_one<T, MPAD, EPI_SWIGLU>(a, b, c, p, s, ch, pf);
-    case EPI_QKV_ROPE: return launch_one<T, MPAD, EPI_QKV_ROPE>(a, b, c, p, s, ch, pf);
-    case EPI_PARTIAL_F32: return launch_one<T, MPAD, EPI_PARTIAL_F32>(a, b, c, p, s, ch, pf);
-    case EPI_SWIGLU_IL: return launch_one<T, MPAD, EPI_SWIGLU_IL>(a, b, c, p, s, ch, pf);
+    case EPI_STORE: return launch_one<T, MPAD, EPI_STORE>(a, b, c, p, s, pf);
+    case EPI_RESIDUAL: return launch_one<T, MPAD, EPI_RESIDUAL>(a, b, c, p, s, pf);
+    case EPI_SWIGLU: return launch_one<T, MPAD, EPI_SWIGLU>(a, b, c, p, s, pf);
+    case EPI_QKV_ROPE: return launch_one<T, MPAD, EPI_QKV_ROPE>(a, b, c, p, s, pf);
+    case EPI_PARTIAL_F32: return launch_one<T, MPAD, EPI_PARTIAL_F32>(a, b, c, p, s, pf);
+    case EPI_SWIGLU_IL: return launch_one<T, MPAD, EPI_SWIGLU_IL>(a, b, c, p, s, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }
@@ -612,15 +570,15 @@ static int launch_epi(int epi, const CUtensorMap* a, const CUtensorMap* b, const
 template <typename T>
 static int launch_epi256(int epi, const CUtensorMap* a, const CUtensorMap* c, const GemmParams& p, cudaStream_t s, const L2Prefetch* pf) {
   switch (epi) {
-    case EPI_RESIDUAL: return launch_one<T, 256, EPI_RESIDUAL>(a, nullptr, c, p, s, nullptr, pf);
-    case EPI_QKV_ROPE: return launch_one<T, 256, EPI_QKV_ROPE>(a, nullptr, c, p, s, nullptr, pf);
-    case EPI_SWIGLU_IL: return launch_one<T, 256, EPI_SWIGLU_IL>(a, nullptr, c, p, s, nullptr, pf);
+    case EPI_RESIDUAL: return launch_one<T, 256, EPI_RESIDUAL>(a, nullptr, c, p, s, pf);
+    case EPI_QKV_ROPE: return launch_one<T, 256, EPI_QKV_ROPE>(a, nullptr, c, p, s, pf);
+    case EPI_SWIGLU_IL: return launch_one<T, 256, EPI_SWIGLU_IL>(a, nullptr, c, p, s, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }
 
 int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX,
-                const GemmParams& p_in, cudaStream_t s, const CUtensorMap* tmXh, const L2Prefetch* pf) {
+                const GemmParams& p_in, cudaStream_t s, const L2Prefetch* pf) {
   GemmParams p = p_in;
   if (p.splitk < 1 || p.m_rows > mpad) return static_cast<int>(cudaErrorInvalidValue);
   if (epi == EPI_SWIGLU || epi == EPI_SWIGLU_IL) {
@@ -628,12 +586,12 @@ int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUte
     if (!p.silu_lut) return static_cast<int>(cudaErrorNotReady);
   }
   if (dtype == DT_BF16) {
-    if (mpad == 16) return launch_epi<__nv_bfloat16, 16>(epi, tmW, tmW2, tmX, p, s, nullptr, pf);
-    if (mpad == 64) return launch_epi<__nv_bfloat16, 64>(epi, tmW, tmW2, tmX, p, s, tmXh, pf);
+    if (mpad == 16) return launch_epi<__nv_bfloat16, 16>(epi, tmW, tmW2, tmX, p, s, pf);
+    if (mpad == 64) return launch_epi<__nv_bfloat16, 64>(epi, tmW, tmW2, tmX, p, s, pf);
     if (mpad == 256) return launch_epi256<__nv_bfloat16>(epi, tmW, tmX, p, s, pf);
   } else if (dtype == DT_FP16) {
-    if (mpad == 16) return launch_epi<__half, 16>(epi, tmW, tmW2, tmX, p, s, nullptr, pf);
-    if (mpad == 64) return launch_epi<__half, 64>(epi, tmW, tmW2, tmX, p, s, tmXh, pf);
+    if (mpad == 16) return launch_epi<__half, 16>(epi, tmW, tmW2, tmX, p, s, pf);
+    if (mpad == 64) return launch_epi<__half, 64>(epi, tmW, tmW2, tmX, p, s, pf);
     if (mpad == 256) return launch_epi256<__half>(epi, tmW, tmX, p, s, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
@@ -645,11 +603,11 @@ static int launch_wq_epi(int epi, const CUtensorMap* w, const CUtensorMap* w2, c
                          const L2Prefetch* pf) {
   switch (epi) {
     case EPI_STORE:
-      if constexpr (MPAD < 256) return launch_one_x<T, MPAD, EPI_STORE, false, WQ>(w, w2, x, x, p, s, pf);
+      if constexpr (MPAD < 256) return launch_one<T, MPAD, EPI_STORE, WQ>(w, w2, x, p, s, pf);
       break;
-    case EPI_RESIDUAL: return launch_one_x<T, MPAD, EPI_RESIDUAL, false, WQ>(w, w2, x, x, p, s, pf);
-    case EPI_QKV_ROPE: return launch_one_x<T, MPAD, EPI_QKV_ROPE, false, WQ>(w, w2, x, x, p, s, pf);
-    case EPI_SWIGLU_IL: return launch_one_x<T, MPAD, EPI_SWIGLU_IL, false, WQ>(w, w2, x, x, p, s, pf);
+    case EPI_RESIDUAL: return launch_one<T, MPAD, EPI_RESIDUAL, WQ>(w, w2, x, p, s, pf);
+    case EPI_QKV_ROPE: return launch_one<T, MPAD, EPI_QKV_ROPE, WQ>(w, w2, x, p, s, pf);
+    case EPI_SWIGLU_IL: return launch_one<T, MPAD, EPI_SWIGLU_IL, WQ>(w, w2, x, p, s, pf);
   }
   return static_cast<int>(cudaErrorInvalidValue);
 }

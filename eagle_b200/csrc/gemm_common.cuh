@@ -1,5 +1,5 @@
-// Tile constants and the epilogue device functions shared by the two wgmma GEMM kernels (cluster split-K in gemm.cu,
-// persistent stream-K in gemm_streamk.cu) and the SIMT bring-up kernel.
+// Tile constants and the epilogue device functions shared by the wgmma GEMM kernel (cluster split-K, gemm.cu) and the SIMT
+// bring-up kernel.
 #pragma once
 #include "common.cuh"
 #include "kernels.h"
@@ -8,7 +8,7 @@ namespace eb {
 
 constexpr int kBlockN = 128;  // weight rows per tile == two wgmma M = 64 halves
 constexpr int kBlockK = 64;   // K elements per stage == one 128-byte swizzle row
-constexpr int kGemmThreads = 288;  // warps 0..7: two MMA warpgroups (gemm.cu) or MMA + epilogue warpgroups (stream-K); warp 8 TMA
+constexpr int kGemmThreads = 288;  // warps 0..7: two MMA warpgroups; warp 8 TMA
 constexpr int kTmaWarp = 8;
 constexpr int kWTileBytes = kBlockN * kBlockK * 2;
 constexpr int kMaxStages = 12;

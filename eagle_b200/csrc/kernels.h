@@ -100,10 +100,8 @@ struct alignas(64) L2Prefetch {
 // Returns cudaError_t-compatible int (0 = ok).  mpad in {16, 64}.  tm* are HOST pointers to encoded maps.
 // pf (optional): after its last weight load, the producer lane of every CTA prefetches its share of that plan (the GEMM that
 // follows), so HBM keeps streaming while this launch drains (cluster reduction, epilogue) and the next kernels ramp.
-// tmXh (optional, mpad == 64): the same activation buffer with a 32-row box -- enables the X-multicast variant (neighbouring n-tiles
-// in a cluster share every X tile, each CTA loads half of it)
 int launch_gemm(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX,
-                const GemmParams& p, cudaStream_t s, const CUtensorMap* tmXh = nullptr, const L2Prefetch* pf = nullptr);
+                const GemmParams& p, cudaStream_t s, const L2Prefetch* pf = nullptr);
 // W8A16 form of launch_gemm: tmW maps an int8 [N][K] weight (make_tmap_w8 layout: box 128 rows x 64 bytes, no swizzle) and
 // p.w_scale its row scales.  The kernel forms W' = T((q * scale) * kInv127) in shared memory and runs the same wgmma sequence and
 // epilogue as launch_gemm, so the result is bit-identical to launch_gemm on W'.  mpad 16 / 64: EPI_STORE, EPI_RESIDUAL,
@@ -140,10 +138,6 @@ int launch_fp8_repack(const uint8_t* src, const float* src_scale, int nr, int K,
 // bring-up / debugging aid: same epilogues, plain FMA main loop, no TMA/wgmma.  W/W2/X are raw pointers.
 int launch_gemm_simt(int dtype, int mpad, int epi, const void* W, const void* W2, const void* X, long ldx,
                      const GemmParams& p, cudaStream_t s);
-// persistent stream-K variant (gemm_streamk.cu): ws >= streamk_ws_bytes(), flags >= one zeroed int per n-tile
-int launch_gemm_streamk(int dtype, int mpad, int epi, const CUtensorMap* tmW, const CUtensorMap* tmW2, const CUtensorMap* tmX,
-                        const GemmParams& p, float* ws, int* flags, cudaStream_t s);
-size_t streamk_ws_bytes();
 // Device table lut[bits(g)] = T(g / (1 + exp(-g))) over all 65536 patterns of the model dtype: the SwiGLU epilogues look the
 // activation up instead of evaluating exp + divide per element (same values by construction).  Built once per device on `s`.
 const void* silu_lut(int dtype, cudaStream_t s);

@@ -65,8 +65,7 @@ typedef struct eb200_config {
 /* The q/k/v/o/gate/up/down projections of every TARGET decoder layer are stored as int8 plus one fp32 scale per row
  * (bitsandbytes' 8-bit weight format) and multiplied by a W8A16 GEMM that computes exactly what the model-dtype GEMM computes on
  * W' = dtype((q * SCB) * 7.874015718698502e-3).  lm_head, embeddings, norms and the draft head stay in the model dtype.
- * Single GPU, default GEMM path only: eb200_finalize refuses tp_size > 1, EB200_FLAG_SIMT_GEMM, EB200_CHAIN=1 and
- * EB200_GEMM_MODE=streamk. */
+ * Single GPU, default GEMM path only: eb200_finalize refuses tp_size > 1, EB200_FLAG_SIMT_GEMM and EB200_CHAIN=1. */
 #define EB200_FLAG_TARGET_INT8 8
 /* The same projections stored as bitsandbytes 4-bit codes (NF4 or FP4 table, blocksize 64: one fp32 absmax per 64 consecutive
  * elements of a row) and multiplied by a W4A16 GEMM that computes exactly what the model-dtype GEMM computes on
@@ -218,7 +217,8 @@ int eb200_get_stats(eb200_engine* e, eb200_stats* out);
 int eb200_reset_stats(eb200_engine* e);
 
 /* ---- per-kernel entry points (parity tests call each kernel in isolation through the same library) ----
- * All pointers are DEVICE pointers unless noted; dtype is EB200_BF16/FP16. */
+ * All pointers are DEVICE pointers unless noted; dtype is EB200_BF16/FP16.
+ * simt (eb200_k_gemm, eb200_k_qkv_rope): 1 runs the SIMT bring-up kernel; 0 and 2 both run the engine's cluster split-K kernel. */
 int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const void* W, const void* W2, const void* X, void* out,
                  const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
 /* the W8A16 cluster split-K GEMM (EB200_FLAG_TARGET_INT8): Wq int8 [N, K], scb fp32 [N]; epilogue codes and M <= 64 as

@@ -67,8 +67,8 @@ GEMM_CASES = [
 ]
 
 
-# kernel selector of the eb200_k_gemm* test entry points: 0 = engine default (persistent stream-K), 1 = SIMT bring-up
-# kernel, 2 = cluster split-K kernel
+# kernel selector of the eb200_k_gemm* test entry points: 0 and 2 = cluster split-K kernel (the engine's), 1 = SIMT
+# bring-up kernel
 MODES = [0, 1, 2]
 
 
