@@ -2833,11 +2833,28 @@ struct Scratch {
   }
 };
 
+// Activation rows a test entry point launches for M rows: 16 or 64 like the cycle, or 256 like the prompt prefill (X is then a
+// [256, K] buffer).  Above 64 rows only what target_prefill runs is accepted -- the wgmma kernel with the residual, interleaved
+// SwiGLU or QKV + RoPE epilogue -- and anything else is refused before an allocation or a launch.
+static int entry_mpad(const char* who, int M, int epilogue, bool simt, int* mpad) {
+  if (M < 1 || M > 256) return fail("%s: M = %d is outside [1, 256]", who, M);
+  if (M <= 64) {
+    *mpad = M <= 16 ? 16 : 64;
+    return 0;
+  }
+  if (simt) return fail("%s: the SIMT kernel runs at most 64 rows (M = %d)", who, M);
+  if (epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL && epilogue != EPI_QKV_ROPE)
+    return fail("%s: epilogue %d is not run at 256 rows (M = %d): only residual, interleaved SwiGLU and QKV + RoPE are", who, epilogue, M);
+  *mpad = 256;
+  return 0;
+}
+
 extern "C" int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const void* W, const void* W2, const void* X, void* out,
                             const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream) {
-  if (M < 1 || M > 64 || epilogue < EPI_STORE || (epilogue > EPI_SWIGLU && epilogue != EPI_SWIGLU_IL)) return fail("eb200_k_gemm: bad arguments");
+  if (epilogue < EPI_STORE || (epilogue > EPI_SWIGLU && epilogue != EPI_SWIGLU_IL)) return fail("eb200_k_gemm: bad arguments");
+  int mpad = 0;
+  TRY(entry_mpad("eb200_k_gemm", M, epilogue, simt == 1, &mpad));
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int mpad = M <= 16 ? 16 : 64;
   Scratch sc;
   const int n_out = N;  // EPI_SWIGLU_IL: W is the [2N, K] interleaved gate/up matrix, out is [M, N]
   if (epilogue == EPI_SWIGLU_IL) {
@@ -2868,7 +2885,7 @@ extern "C" int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const
     CUtensorMap tw, tw2, tx;
     TRY(make_tmap(&tw, dtype, W, N, K, 128));
     if (W2) TRY(make_tmap(&tw2, dtype, W2, N, K, 128));
-    TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
+    TRY(make_tmap(&tx, dtype, X, std::max(64, mpad), K, mpad));
     if (p.splitk > 8) p.splitk = 8;
     CKL(launch_gemm(dtype, mpad, epilogue, &tw, W2 ? &tw2 : nullptr, &tx, p, s));
   }
@@ -2917,11 +2934,11 @@ extern "C" int eb200_k_prefetch(int32_t dtype, int32_t kernel, int32_t epilogue,
 
 extern "C" int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, const void* scb, const void* X, void* out, const void* res,
                                const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream) {
-  if (M < 1 || M > 64 || (epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !scb || splitk < 1 ||
-      splitk > 8)
+  if ((epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !scb || splitk < 1 || splitk > 8)
     return fail("eb200_k_gemm_w8: bad arguments");
+  int mpad = 0;
+  TRY(entry_mpad("eb200_k_gemm_w8", M, epilogue, false, &mpad));
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int mpad = M <= 16 ? 16 : 64;
   const int n_out = N;  // EPI_SWIGLU_IL: Wq is the [2N, K] interleaved gate/up matrix, out is [M, N]
   if (epilogue == EPI_SWIGLU_IL) {
     if (N % 64) return fail("eb200_k_gemm_w8: interleaved SwiGLU needs N % 64 == 0");
@@ -2942,7 +2959,7 @@ extern "C" int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, 
   p.w_scale = reinterpret_cast<const float*>(scb);
   CUtensorMap tw, tx;
   TRY(make_tmap_w8(&tw, Wq, N, K));
-  TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
+  TRY(make_tmap(&tx, dtype, X, std::max(64, mpad), K, mpad));
   CKL(launch_gemm_w8(dtype, mpad, epilogue, &tw, &tx, p, s));
   CK(cudaStreamSynchronize(s));
   return 0;
@@ -2950,11 +2967,12 @@ extern "C" int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, 
 
 extern "C" int eb200_k_gemm_w4(int32_t dtype, int32_t quant_type, int32_t epilogue, const void* Wq, const void* absmax, const void* X, void* out,
                                const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream) {
-  if (M < 1 || M > 64 || (epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !absmax || splitk < 1 ||
-      splitk > 8 || N < 1 || K < 64 || K % 64 || (quant_type != W4_NF4 && quant_type != W4_FP4))
+  if ((epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !absmax || splitk < 1 || splitk > 8 ||
+      N < 1 || K < 64 || K % 64 || (quant_type != W4_NF4 && quant_type != W4_FP4))
     return fail("eb200_k_gemm_w4: bad arguments");
+  int mpad = 0;
+  TRY(entry_mpad("eb200_k_gemm_w4", M, epilogue, false, &mpad));
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int mpad = M <= 16 ? 16 : 64;
   const int n_out = N;  // EPI_SWIGLU_IL: Wq is the [2N, K/2] interleaved gate/up matrix, out is [M, N]
   if (epilogue == EPI_SWIGLU_IL) {
     if (N % 64) return fail("eb200_k_gemm_w4: interleaved SwiGLU needs N % 64 == 0");
@@ -2985,7 +3003,7 @@ extern "C" int eb200_k_gemm_w4(int32_t dtype, int32_t quant_type, int32_t epilog
       launch_w4_repack(static_cast<const uint8_t*>(Wq), static_cast<const float*>(absmax), N, K, 0, -1, tiles, am, n_pad, s) != 0)
     rc = fail("eb200_k_gemm_w4: repack failed");
   if (!rc) rc = make_tmap_w4(&tw, &ta, tiles, am, n_pad, K);
-  if (!rc) rc = make_tmap(&tx, dtype, X, 64, K, mpad);
+  if (!rc) rc = make_tmap(&tx, dtype, X, std::max(64, mpad), K, mpad);
   if (!rc) {
     const int r = launch_gemm_w4(dtype, mpad, epilogue, &tw, &ta, &tx, p, s);
     if (r != 0) rc = fail("eb200_k_gemm_w4: launch failed (%d)", r);
@@ -2997,11 +3015,12 @@ extern "C" int eb200_k_gemm_w4(int32_t dtype, int32_t quant_type, int32_t epilog
 
 extern "C" int eb200_k_gemm_fp8(int32_t dtype, int32_t epilogue, const void* Wq, const void* scale_inv, const void* X, void* out,
                                 const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream) {
-  if (M < 1 || M > 64 || (epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !scale_inv || splitk < 1 ||
-      splitk > 8 || N < 1 || K < 128 || K % 128)
+  if ((epilogue != EPI_STORE && epilogue != EPI_RESIDUAL && epilogue != EPI_SWIGLU_IL) || !Wq || !scale_inv || splitk < 1 || splitk > 8 ||
+      N < 1 || K < 128 || K % 128)
     return fail("eb200_k_gemm_fp8: bad arguments");
+  int mpad = 0;
+  TRY(entry_mpad("eb200_k_gemm_fp8", M, epilogue, false, &mpad));
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int mpad = M <= 16 ? 16 : 64;
   const int n_out = N;  // EPI_SWIGLU_IL: Wq is the [2N, K] interleaved gate/up matrix, out is [M, N]
   if (epilogue == EPI_SWIGLU_IL) N *= 2;
   if (N % 128) return fail("eb200_k_gemm_fp8: the weight's rows (%d) must be a multiple of 128", N);
@@ -3028,7 +3047,7 @@ extern "C" int eb200_k_gemm_fp8(int32_t dtype, int32_t epilogue, const void* Wq,
       launch_fp8_repack(static_cast<const uint8_t*>(Wq), static_cast<const float*>(scale_inv), N, K, 0, -1, q, sc, N, s) != 0)
     rc = fail("eb200_k_gemm_fp8: repack failed");
   if (!rc) rc = make_tmap_fp8(&tw, &ts, q, sc, N, K);
-  if (!rc) rc = make_tmap(&tx, dtype, X, 64, K, mpad);
+  if (!rc) rc = make_tmap(&tx, dtype, X, std::max(64, mpad), K, mpad);
   if (!rc) {
     const int r = launch_gemm_fp8(dtype, mpad, epilogue, &tw, &ts, &tx, p, s);
     if (r != 0) rc = fail("eb200_k_gemm_fp8: launch failed (%d)", r);
@@ -3220,9 +3239,10 @@ extern "C" int eb200_k_gemm_bench(int32_t dtype, int32_t epilogue, int32_t M, in
 extern "C" int eb200_k_qkv_rope(int32_t dtype, int32_t simt, const void* Wqkv, const void* X, void* q_out, void* k_cache, void* v_cache,
                                 const void* cosp, const void* sinp, const int32_t* pos, int32_t M, int32_t n_heads, int32_t n_kv_heads,
                                 int32_t K, int64_t kv_cap, int32_t kv_base, int32_t splitk, void* stream) {
-  if (M < 1 || M > 64) return fail("eb200_k_qkv_rope: bad M");
+  int mpad = 0;
+  TRY(entry_mpad("eb200_k_qkv_rope", M, EPI_QKV_ROPE, simt == 1, &mpad));
+  if (kv_base < 0 || kv_base + M > kv_cap) return fail("eb200_k_qkv_rope: cache rows [%d, %d) outside [0, %lld)", kv_base, kv_base + M, (long long)kv_cap);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int mpad = M <= 16 ? 16 : 64;
   const int N = (n_heads + 2 * n_kv_heads) * 128;
   Scratch sc;
   const int tiles = N / 128;
@@ -3246,16 +3266,17 @@ extern "C" int eb200_k_qkv_rope(int32_t dtype, int32_t simt, const void* Wqkv, c
   p.n_kv_heads = n_kv_heads;
   p.rope_cos = cosp;
   p.rope_sin = sinp;
-  p.pos_base = DynInt{-1, 0};
+  // pos[m]: the cycle's form (tree positions); no pos: the prefill's (chunk_ctx), row m at position kv_base + m
+  p.pos_base = DynInt{-1, pos ? 0 : kv_base};
   p.pos_arr = pos;
-  p.pos_mstride = 0;
+  p.pos_mstride = pos ? 0 : 1;
   p.kv_base = DynInt{-1, kv_base};
   if (simt == 1) {
     CKL(launch_gemm_simt(dtype, mpad, EPI_QKV_ROPE, Wqkv, nullptr, X, K, p, s));
   } else {
     CUtensorMap tw, tx;
     TRY(make_tmap(&tw, dtype, Wqkv, N, K, 128));
-    TRY(make_tmap(&tx, dtype, X, 64, K, mpad));
+    TRY(make_tmap(&tx, dtype, X, std::max(64, mpad), K, mpad));
     if (p.splitk > 8) p.splitk = 8;
     CKL(launch_gemm(dtype, mpad, EPI_QKV_ROPE, &tw, nullptr, &tx, p, s));
   }

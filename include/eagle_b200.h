@@ -218,10 +218,13 @@ int eb200_reset_stats(eb200_engine* e);
 
 /* ---- per-kernel entry points (parity tests call each kernel in isolation through the same library) ----
  * All pointers are DEVICE pointers unless noted; dtype is EB200_BF16/FP16.
- * simt (eb200_k_gemm, eb200_k_qkv_rope): 1 runs the SIMT bring-up kernel; 0 and 2 both run the engine's cluster split-K kernel. */
+ * simt (eb200_k_gemm, eb200_k_qkv_rope): 1 runs the SIMT bring-up kernel; 0 and 2 both run the engine's cluster split-K kernel.
+ * Rows (eb200_k_gemm*, eb200_k_qkv_rope): 1 <= M <= 64 launches 16 or 64 activation rows and X is a [64, K] buffer; 64 < M <= 256
+ * launches the prompt prefill's 256 rows and X is a [256, K] buffer.  Above 64 rows only the cluster kernel with the residual (1),
+ * interleaved SwiGLU (5) and QKV + RoPE epilogues runs; store, two-matrix SwiGLU and the SIMT kernel are refused. */
 int eb200_k_gemm(int32_t dtype, int32_t simt, int32_t epilogue, const void* W, const void* W2, const void* X, void* out,
                  const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
-/* the W8A16 cluster split-K GEMM (EB200_FLAG_TARGET_INT8): Wq int8 [N, K], scb fp32 [N]; epilogue codes and M <= 64 as
+/* the W8A16 cluster split-K GEMM (EB200_FLAG_TARGET_INT8): Wq int8 [N, K], scb fp32 [N]; epilogue codes and M as
  * eb200_k_gemm (0 store, 1 residual, 5 interleaved SwiGLU with N output columns over a [2N, K] weight); bias: store only */
 int eb200_k_gemm_w8(int32_t dtype, int32_t epilogue, const void* Wq, const void* scb, const void* X, void* out, const void* res,
                     const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
@@ -272,6 +275,9 @@ int eb200_k_attention_ex(int32_t dtype, const void* q, const void* k_cache, cons
                          int32_t n_heads, int32_t n_kv_heads, int64_t kv_cap, int32_t max_kv, const int32_t* st, int32_t rows_idx,
                          int32_t n_ctx_idx, int32_t n_ctx_add, int32_t n_tree, const uint64_t* mask, int32_t hpc_cap,
                          int32_t kvs_cap, void* stream);
+/* X . Wqkv^T with RoPE: q_out [M, n_heads * 128], K / V rows [kv_base, kv_base + M) of the [n_kv_heads, kv_cap, 128] caches;
+ * cos / sin [positions, 64].  Row m is rotated to position pos[m] (the cycle's form), or to kv_base + m when pos is null (the
+ * prompt prefill's form). */
 int eb200_k_qkv_rope(int32_t dtype, int32_t simt, const void* Wqkv, const void* X, void* q_out, void* k_cache,
                      void* v_cache, const void* cos, const void* sin, const int32_t* pos, int32_t M, int32_t n_heads,
                      int32_t n_kv_heads, int32_t K, int64_t kv_cap, int32_t kv_base, int32_t splitk, void* stream);

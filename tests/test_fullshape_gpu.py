@@ -107,3 +107,21 @@ def test_draft_logits_within_1e3_of_the_oracle(pair):
         worst = max(worst, float((err / (1e-3 + ULP_BF16 * want[j].abs())).max()))
     report(f"full-shape draft logits ({len(pairs)} comparable frontier rows): {n_bad}/{n_all} elements beyond 1e-3 + 1 ulp; worst error {worst:.2f} x tolerance")
     assert n_bad <= n_all * 1e-3 and worst <= 3.0, f"{n_bad}/{n_all} draft logits beyond 1e-3 + 1 bf16 ulp; worst {worst:.2f}x"
+
+
+def test_prefill_kv_within_the_oracle_bars_at_llama3_8b_width(pair):
+    """The 700-token prompt runs as 256 + 256 + 188 rows through the 256-row GEMMs at H = 4096.  The bigram target's margins
+    keep the generated ids unchanged under a wrong K/V row, so the target KV itself is held to the oracle's, with the bars of
+    tests/test_prefill_gpu.py."""
+    from tests.test_prefill_gpu import by_block, kv_bars, planes, target_rope_terms
+    m, ref, prompt = pair
+    kv = ref._kv(1100)
+    ref.target.forward(prompt, kv)
+    want = kv.data[:, 0, :, :P].float().reshape(-1, P, 128)
+    m.prefill(prompt.cuda())
+    got = planes(m, "target_kv", P)
+    fails, rows, worst = kv_bars(got, want, 2 * ref.target.cfg.num_key_value_heads, torch.bfloat16, "target KV",
+                                 target_rope_terms(ref, prompt))
+    report(f"full-shape prefill (P = {P}): worst row distance to the oracle per 64-row block of a 256-row chunk {by_block(rows)}; "
+           f"layer-0 worst {worst:.2f} x (1e-3 + 2 ulp)")
+    assert not fails, "; ".join(fails)

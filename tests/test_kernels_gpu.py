@@ -43,6 +43,19 @@ def close(got, want, dtype, what=""):
         raise AssertionError(msg)
 
 
+def close_rope(got, x, cos, sin, pos, want, dtype, what=""):
+    """RoPE outputs T(T(x c) + T(rotate_half(x) s)) of the rounded projection x [heads, M, 128] at positions pos: 1e-3 plus one
+    ulp of the output plus two of each product.  The kernel rounds the same products as the reference, but a one-ulp flip of x
+    (or of its rotation partner) moves a product by an ulp of it, and where the two products cancel that is many ulps of the
+    output (long K sums and large angles make such flips and cancellations common)."""
+    c, s, x = cos[pos].float(), sin[pos].float(), x.float()
+    terms = (x * c).abs() + (orc._rotate_half(x) * s).abs()
+    got, want = got.float().cpu(), want.float().cpu()
+    bad = (got - want).abs() > 1e-3 + ULP[dtype] * (want.abs() + 2 * terms)
+    assert not bad.any(), (f"{what}: {int(bad.sum())}/{bad.numel()} elements out of tolerance; first bad {bad.nonzero()[:8].tolist()}; "
+                           f"got {got[bad][:8].tolist()} want {want[bad][:8].tolist()}")
+
+
 _KEEP = []
 
 
@@ -72,6 +85,19 @@ GEMM_CASES = [
 MODES = [0, 1, 2]
 
 
+def x_rows(M):
+    """Rows of the activation buffer the test entry points read for M rows: 64, or 256 for the prompt prefill's launch."""
+    return 256 if M > 64 else 64
+
+
+# Above 64 rows the kernel runs the prompt prefill's 256-row instantiation (wgmma N = 256): 65 is its smallest launch; with
+# splitk 3 each CTA reduces 86 rows, so a CTA's last 16-row chunk is partial; at M = 100 and splitk 8 ranks 4..7 own no valid row.
+PREFILL_CASES = [  # M, N, K, splitk
+    (65, 256, 512, 1), (70, 384, 768, 3), (128, 512, 512, 2), (129, 256, 1024, 8), (192, 640, 256, 4), (255, 384, 768, 3),
+    (256, 1024, 512, 1), (256, 512, 1024, 8), (100, 256, 1024, 8),
+]
+
+
 @pytest.mark.parametrize("simt", MODES)
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("M,N,K,splitk", GEMM_CASES)
@@ -94,22 +120,34 @@ def test_gemm_store(lib, M, N, K, splitk, dtype, simt):
 @pytest.mark.parametrize("M,N,K,splitk,epi", [
     (60, 6144, 4096, 4, "qkv"), (60, 4096, 4096, 8, "res"), (60, 14336, 4096, 2, "swiglu"), (60, 4096, 14336, 8, "res"),
     (60, 128256, 4096, 1, "store"), (10, 32000, 4096, 1, "store"), (10, 6144, 8192, 4, "store"), (8, 4096, 12288, 8, "store"),
+    # a full 256-row prompt chunk: Llama-3-8B qkv / o / gate_up / down, Llama-3-70B o / down
+    (256, 6144, 4096, 4, "qkv"), (256, 4096, 4096, 4, "res"), (256, 14336, 4096, 1, "swiglu"), (256, 4096, 14336, 4, "res"),
+    (256, 8192, 8192, 2, "res"), (256, 8192, 28672, 2, "res"),
 ])
 @pytest.mark.parametrize("mode", [0, 2])
 def test_gemm_llama3_8b_shapes(lib, M, N, K, splitk, epi, mode):
-    """The projections of the benchmark configuration (BASELINE.json configs[1..2]) at full size, checked against a
-    float64 reference on sampled output columns (size-independent property: linearity in W rows)."""
+    """The projections of the benchmark configuration (BASELINE.json configs[1..2]) at full size, and those of a 256-row
+    prompt chunk of Llama-3-8B and -70B, checked against a float64 reference on sampled output columns (size-independent
+    property: linearity in W rows).  At 256 rows the prefill's epilogues run: gate/up interleaved, and qkv through the
+    QKV + RoPE epilogue with an identity rotation (cos 1, sin 0), which makes it a store into q and the K / V caches (the
+    rotation itself is held to the reference by test_qkv_rope_kv_append)."""
     dtype = torch.bfloat16
+    R = x_rows(M)
     g = torch.Generator(device="cuda").manual_seed(N + K)
-    X = (torch.randn(64, K, generator=g, device="cuda") * 0.5).to(dtype)
+    X = (torch.randn(R, K, generator=g, device="cuda") * 0.5).to(dtype)
     W = (torch.randn(N, K, generator=g, device="cuda") * 0.02).to(dtype)
     cols = torch.randint(0, N, (512,), generator=torch.Generator().manual_seed(3)).cuda()
     torch.cuda.synchronize()
     if epi == "swiglu":
         W2 = (torch.randn(N, K, generator=g, device="cuda") * 0.02).to(dtype)
         torch.cuda.synchronize()
-        out = torch.zeros(64, N, dtype=dtype, device="cuda")
-        check(lib, lib.eb200_k_gemm(0, mode, 2, ptr(W), ptr(W2), ptr(X), ptr(out), None, None, M, N, K, splitk, None))
+        out = torch.zeros(R, N, dtype=dtype, device="cuda")
+        if M > 64:
+            Wil = interleave64(W, W2)
+            torch.cuda.synchronize()
+            check(lib, lib.eb200_k_gemm(0, mode, 5, ptr(Wil), None, ptr(X), ptr(out), None, None, M, N, K, splitk, None))
+        else:
+            check(lib, lib.eb200_k_gemm(0, mode, 2, ptr(W), ptr(W2), ptr(X), ptr(out), None, None, M, N, K, splitk, None))
         gate = (X[:M].double() @ W[cols].double().t()).to(dtype)
         up = (X[:M].double() @ W2[cols].double().t()).to(dtype)
         want = F.silu(gate) * up
@@ -117,12 +155,25 @@ def test_gemm_llama3_8b_shapes(lib, M, N, K, splitk, epi, mode):
         tol = 1e-3 + 3.2 * ULP[dtype] * want.float().abs() + ULP[dtype] * up.float().abs() * 0.02
         assert bool((err <= tol).all()), f"max err {float(err.max())}"
         return
-    res = torch.randn(64, N, generator=g, device="cuda").to(dtype) if epi == "res" else None
+    res = torch.randn(R, N, generator=g, device="cuda").to(dtype) if epi == "res" else None
     torch.cuda.synchronize()
-    out = res.clone() if res is not None else torch.zeros(64, N, dtype=dtype, device="cuda")
+    out = res.clone() if res is not None else torch.zeros(R, N, dtype=dtype, device="cuda")
     torch.cuda.synchronize()
-    code = 1 if epi == "res" else 0
-    check(lib, lib.eb200_k_gemm(0, mode, code, ptr(W), None, ptr(X), ptr(out), ptr(out) if res is not None else None, None, M, N, K, splitk, None))
+    if epi == "qkv" and M > 64:
+        nkv = 8
+        nh = N // 128 - 2 * nkv  # Llama-3-8B: 32 query heads, 8 kv heads
+        cos = torch.ones(M, 64, dtype=dtype, device="cuda")
+        kc = torch.zeros(nkv, M, 128, dtype=dtype, device="cuda")
+        vc = torch.zeros(nkv, M, 128, dtype=dtype, device="cuda")
+        q_out = torch.zeros(R, nh * 128, dtype=dtype, device="cuda")
+        torch.cuda.synchronize()
+        check(lib, lib.eb200_k_qkv_rope(0, mode, ptr(W), ptr(X), ptr(q_out), ptr(kc), ptr(vc), ptr(cos), ptr(torch.zeros_like(cos)), None,
+                                        M, nh, nkv, K, M, 0, splitk, None))
+        out = torch.cat((q_out[:M], kc.transpose(0, 1).reshape(M, -1), vc.transpose(0, 1).reshape(M, -1)), dim=1)
+    else:
+        code = 1 if epi == "res" else 0
+        check(lib, lib.eb200_k_gemm(0, mode, code, ptr(W), None, ptr(X), ptr(out), ptr(out) if res is not None else None, None, M, N, K,
+                                    splitk, None))
     proj = (X[:M].double() @ W[cols].double().t()).to(dtype)
     want = (res[:M][:, cols] + proj) if res is not None else proj
     err = (out[:M][:, cols].float() - want.float()).abs()
@@ -139,12 +190,16 @@ def interleave64(Wg, Wu):
 
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("M,N,K,splitk", [(10, 512, 256, 1), (60, 1024, 256, 2), (60, 1408, 512, 1), (60, 1792, 4096, 4), (7, 64, 256, 1)])
+@pytest.mark.parametrize("M,N,K,splitk", [(10, 512, 256, 1), (60, 1024, 256, 2), (60, 1408, 512, 1), (60, 1792, 4096, 4), (7, 64, 256, 1)]
+                         + [(M, 64 * (N // 128), K, sk) for M, N, K, sk in PREFILL_CASES])
 def test_gemm_swiglu_interleaved(lib, M, N, K, splitk, dtype, mode):
     """Single-accumulator SwiGLU over interleaved gate/up rows: same rounding points as the two-matrix kernel, so the two
-    must agree BIT FOR BIT (same fp32 accumulation order per element), and both sit within tolerance of the torch reference."""
+    must agree BIT FOR BIT (same fp32 accumulation order per element), and both sit within tolerance of the torch reference.
+    Above 64 rows (the prefill's 256-row launch, which has no two-matrix form) only the reference bar applies."""
+    if mode == 1 and M > 64:
+        pytest.skip("the SIMT bring-up kernel runs at most 64 rows")
     g = torch.Generator().manual_seed(12 + N)
-    X = (torch.randn(64, K, generator=g)).to(dtype)
+    X = (torch.randn(x_rows(M), K, generator=g)).to(dtype)
     Wg = (torch.randn(N, K, generator=g) * 0.08).to(dtype)
     Wu = (torch.randn(N, K, generator=g) * 0.08).to(dtype)
     gate = F.linear(X[:M].float(), Wg.float()).to(dtype)
@@ -152,15 +207,15 @@ def test_gemm_swiglu_interleaved(lib, M, N, K, splitk, dtype, mode):
     want = F.silu(gate) * up
     Wil = interleave64(Wg, Wu).cuda()
     Xd = X.cuda()
-    out = torch.zeros(64, N, dtype=dtype, device="cuda")
+    out = torch.zeros(x_rows(M), N, dtype=dtype, device="cuda")
     torch.cuda.synchronize()
     check(lib, lib.eb200_k_gemm(DT[dtype], mode, 5, ptr(Wil), None, ptr(Xd), ptr(out), None, None, M, N, K, splitk, None))
     err = (out[:M].float().cpu() - want.float()).abs()
     tol = 1e-3 + 3.2 * ULP[dtype] * want.float().abs() + ULP[dtype] * up.float().abs() * 0.02
     assert bool((err <= tol).all()), f"gemm_swiglu_il: {int((err > tol).sum())} bad, max err {float(err.max())}"
-    if M < 64:
+    if M < out.shape[0]:
         assert float(out[M:].abs().max()) == 0.0
-    if mode != 1 and N % 128 == 0:
+    if mode != 1 and N % 128 == 0 and M <= 64:
         out2 = torch.zeros(64, N, dtype=dtype, device="cuda")
         Wgd, Wud = Wg.cuda(), Wu.cuda()
         torch.cuda.synchronize()
@@ -212,12 +267,12 @@ def test_gemm_onehot_layout(lib, simt):
 
 @pytest.mark.parametrize("mode", [0, 2])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("M,N,K,splitk", [(10, 256, 512, 1), (60, 512, 256, 2), (60, 4096, 1024, 4)])
+@pytest.mark.parametrize("M,N,K,splitk", [(10, 256, 512, 1), (60, 512, 256, 2), (60, 4096, 1024, 4)] + PREFILL_CASES)
 def test_gemm_residual(lib, M, N, K, splitk, dtype, mode):
     g = torch.Generator().manual_seed(11)
-    X = (torch.randn(64, K, generator=g) * 0.5).to(dtype)
+    X = (torch.randn(x_rows(M), K, generator=g) * 0.5).to(dtype)
     W = (torch.randn(N, K, generator=g) * 0.05).to(dtype)
-    res = torch.randn(64, N, generator=g).to(dtype)
+    res = torch.randn(x_rows(M), N, generator=g).to(dtype)
     proj = F.linear(X[:M].float(), W.float()).to(dtype)
     want = res[:M] + proj  # x + o_proj(a): two roundings
     out = res.clone().cuda()
@@ -226,7 +281,33 @@ def test_gemm_residual(lib, M, N, K, splitk, dtype, mode):
     err = (out[:M].float().cpu() - want.float()).abs()
     tol = 1e-3 + ULP[dtype] * (proj.float().abs() + want.float().abs())
     assert bool((err <= tol).all()), f"gemm_residual: {int((err > tol).sum())} bad, max err {float(err.max())}"
-    assert torch.equal(out[M:].cpu(), res[M:])
+    assert torch.equal(out[M:].cpu(), res[M:])  # rows beyond M are never written
+
+
+def test_gemm_and_qkv_rope_refuse_what_the_prefill_does_not_run_at_256_rows(lib):
+    """Above 64 rows the entry points run only what the prompt prefill runs; everything else fails before any launch, so the
+    output buffer keeps its contents."""
+    dtype = torch.bfloat16
+    N, K = 256, 256
+    W, X = torch.zeros(3 * 128, K, dtype=dtype, device="cuda"), torch.zeros(256, K, dtype=dtype, device="cuda")  # W: N rows, or q/k/v heads
+    out = torch.full((256, N), 7.0, dtype=dtype, device="cuda")
+    torch.cuda.synchronize()
+    refused = {  # what: (simt, epilogue, W2, M)
+        "store": (0, 0, None, 65), "two-matrix SwiGLU": (0, 2, W, 65), "fp32 partials": (0, 4, None, 65),
+        "SIMT kernel": (1, 1, None, 65), "M > 256": (0, 1, None, 257), "M = 0": (0, 1, None, 0),
+    }
+    for what, (simt, epi, W2, M) in refused.items():
+        rc = lib.eb200_k_gemm(0, simt, epi, ptr(W), ptr(W2), ptr(X), ptr(out), ptr(out), None, M, N, K, 1, None)
+        assert rc != 0, f"eb200_k_gemm ran {what}"
+        assert lib.eb200_last_error().decode(), what
+    cos = torch.ones(2048, 64, dtype=dtype, device="cuda")
+    kc = torch.full((1, 1024, 128), 7.0, dtype=dtype, device="cuda")
+    for what, (simt, M, kv_base) in {"SIMT kernel": (1, 65, 0), "M > 256": (0, 257, 0), "cache rows past kv_cap": (0, 200, 900)}.items():
+        rc = lib.eb200_k_qkv_rope(0, simt, ptr(W), ptr(X), ptr(out), ptr(kc), ptr(kc), ptr(cos), ptr(cos), None, M, 1, 1, K, 1024,
+                                  kv_base, 1, None)
+        assert rc != 0, f"eb200_k_qkv_rope ran {what}"
+    torch.cuda.synchronize()
+    assert bool((out == 7.0).all()) and bool((kc == 7.0).all()), "a refused call wrote its output"
 
 
 @pytest.mark.parametrize("mode", [0, 2])
@@ -248,34 +329,99 @@ def test_gemm_swiglu(lib, M, N, K, splitk, dtype, mode):
     assert bool((err <= tol).all()), f"gemm_swiglu: {int((err > tol).sum())} bad, max err {float(err.max())}"
 
 
+QKV_CASES = [  # M, nh, nkv, K, splitk, kv_base, position form: "pos" = pos[m] (the cycle's), "prefill" = kv_base + m
+    pytest.param(10, 2, 1, 256, 1, 37, "pos", id="10-2-1-256-1"), pytest.param(60, 4, 2, 512, 2, 37, "pos", id="60-4-2-512-2"),
+    pytest.param(7, 2, 2, 512, 1, 37, "pos", id="7-2-2-512-1"),
+    # the prompt prefill's 256-row launch, kv_base 0 / 256 / past 1000 in both position forms
+    (65, 2, 1, 256, 1, 0, "prefill"), (70, 2, 2, 512, 3, 256, "pos"), (128, 4, 2, 512, 2, 1029, "prefill"), (129, 2, 1, 1024, 8, 0, "pos"),
+    (192, 2, 2, 256, 4, 256, "prefill"), (255, 4, 2, 768, 3, 1029, "pos"), (256, 2, 1, 512, 1, 1029, "prefill"),
+    (100, 2, 1, 1024, 8, 256, "pos"), (256, 4, 1, 1024, 8, 0, "prefill"),
+]
+
+
 @pytest.mark.parametrize("simt", MODES)
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("M,nh,nkv,K,splitk", [(10, 2, 1, 256, 1), (60, 4, 2, 512, 2), (7, 2, 2, 512, 1)])
-def test_qkv_rope_kv_append(lib, M, nh, nkv, K, splitk, dtype, simt):
+@pytest.mark.parametrize("M,nh,nkv,K,splitk,kv_base,form", QKV_CASES)
+def test_qkv_rope_kv_append(lib, M, nh, nkv, K, splitk, kv_base, form, dtype, simt):
+    if simt == 1 and M > 64:
+        pytest.skip("the SIMT bring-up kernel runs at most 64 rows")
+    R = x_rows(M)
     g = torch.Generator().manual_seed(13)
-    X = torch.randn(64, K, generator=g).to(dtype)
+    X = torch.randn(R, K, generator=g).to(dtype)
     Wq = (torch.randn(nh * 128, K, generator=g) * 0.06).to(dtype)
     Wk = (torch.randn(nkv * 128, K, generator=g) * 0.06).to(dtype)
     Wv = (torch.randn(nkv * 128, K, generator=g) * 0.06).to(dtype)
-    cap, kv_base = 256, 37
-    pos = torch.randint(0, 200, (64,), generator=g, dtype=torch.int32)
-    cos, sin = orc.rope_table(128, 256, 500000.0)
+    n_pos = 2048
+    cap = 256 if M <= 64 else 1536
+    pos = torch.randint(0, 200 if M <= 64 else n_pos, (R,), generator=g, dtype=torch.int32)
+    if form == "prefill":
+        pos = torch.arange(kv_base, kv_base + R, dtype=torch.int32)
+    cos, sin = orc.rope_table(128, n_pos, 500000.0)
     cosT, sinT = cos.to(dtype), sin.to(dtype)
     q = F.linear(X[:M].float(), Wq.float()).to(dtype).view(1, M, nh, 128).transpose(1, 2)
     k = F.linear(X[:M].float(), Wk.float()).to(dtype).view(1, M, nkv, 128).transpose(1, 2)
     v = F.linear(X[:M].float(), Wv.float()).to(dtype).view(1, M, nkv, 128).transpose(1, 2)
     qr, kr = orc.apply_rope(q, k, cosT, sinT, pos[:M].long()[None])
     Wqkv = torch.cat([Wq, Wk, Wv]).cuda()
-    q_out = torch.zeros(64, nh * 128, dtype=dtype, device="cuda")
+    q_out = torch.zeros(R, nh * 128, dtype=dtype, device="cuda")
     kc = torch.zeros(nkv, cap, 128, dtype=dtype, device="cuda")
     vc = torch.zeros(nkv, cap, 128, dtype=dtype, device="cuda")
     check(lib, lib.eb200_k_qkv_rope(DT[dtype], simt, ptr(Wqkv), ptr(X.cuda()), ptr(q_out), ptr(kc), ptr(vc),
                                     ptr(cosT[:, :64].contiguous().cuda()), ptr(sinT[:, :64].contiguous().cuda()),
-                                    ptr(pos.cuda()), M, nh, nkv, K, cap, kv_base, splitk, None))
-    close(q_out[:M].view(M, nh, 128).transpose(0, 1), qr[0], dtype, "q rope")
-    close(kc[:, kv_base:kv_base + M], kr[0], dtype, "k rope/cache")
+                                    ptr(pos.cuda()) if form == "pos" else None, M, nh, nkv, K, cap, kv_base, splitk, None))
+    if M <= 64:  # the cycle-form cases keep the plain 1-ulp bar they were written with
+        close(q_out[:M].view(M, nh, 128).transpose(0, 1), qr[0], dtype, "q rope")
+        close(kc[:, kv_base:kv_base + M], kr[0], dtype, "k rope/cache")
+    else:
+        close_rope(q_out[:M].view(M, nh, 128).transpose(0, 1), q[0], cosT, sinT, pos[:M].long(), qr[0], dtype, "q rope")
+        close_rope(kc[:, kv_base:kv_base + M], k[0], cosT, sinT, pos[:M].long(), kr[0], dtype, "k rope/cache")
     close(vc[:, kv_base:kv_base + M], v[0], dtype, "v cache")
-    assert float(kc[:, :kv_base].abs().max()) == 0 and float(kc[:, kv_base + M:].abs().max()) == 0
+    # cache rows outside [kv_base, kv_base + M) and q rows beyond M are never written
+    for t in (kc[:, :kv_base], kc[:, kv_base + M:], vc[:, :kv_base], vc[:, kv_base + M:], q_out[M:]):
+        assert not bool(t.any())
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+@pytest.mark.parametrize("epi", ["residual", "swiglu", "qkv_rope"])
+def test_256_rows_equal_64_row_launches_bit_for_bit(lib, epi, dtype):
+    """One 256-row launch over rows [0, M) against separate launches (64 or 16 rows, like the 64-row prompt chunks and the cycle)
+    on each 64-row block of X, with the same splitk: each output element sums the same products in the same k-block and rank
+    order, so the two must agree bit for bit.  This is what makes the engine's 256-row and 64-row prefills identical."""
+    g = torch.Generator(device="cuda").manual_seed(21)
+    K, nh, nkv, kv_base = 1024, 4, 2, 300
+    N = {"residual": 1024, "swiglu": 512, "qkv_rope": (nh + 2 * nkv) * 128}[epi]
+    rows = 2 * N if epi == "swiglu" else N
+    X = torch.randn(256, K, generator=g, device="cuda").to(dtype)
+    W = (torch.randn(rows, K, generator=g, device="cuda") * 0.05).to(dtype)
+    res = torch.randn(256, N, generator=g, device="cuda").to(dtype)
+    cos, sin = (t.to(dtype)[:, :64].contiguous().cuda() for t in orc.rope_table(128, 1024, 500000.0))
+    torch.cuda.synchronize()
+
+    def run(r0, M, splitk, out, q_out, kc, vc):
+        """Rows [r0, r0 + M) of X in one launch."""
+        x = ptr(X[r0:])
+        if epi == "qkv_rope":
+            return lib.eb200_k_qkv_rope(DT[dtype], 0, ptr(W), x, ptr(q_out[r0:]), ptr(kc), ptr(vc), ptr(cos), ptr(sin), None, M, nh, nkv,
+                                        K, 1024, kv_base + r0, splitk, None)
+        if epi == "residual":
+            return lib.eb200_k_gemm(DT[dtype], 0, 1, ptr(W), None, x, ptr(out[r0:]), ptr(out[r0:]), None, M, N, K, splitk, None)
+        return lib.eb200_k_gemm(DT[dtype], 0, 5, ptr(W), None, x, ptr(out[r0:]), None, None, M, N, K, splitk, None)
+
+    for M, splitk in [(256, 1), (256, 4), (200, 2), (129, 3), (65, 8), (100, 8)]:
+        results = []
+        for blocks in (False, True):
+            out = res.clone() if epi == "residual" else torch.zeros(256, N, dtype=dtype, device="cuda")
+            q_out = torch.zeros(256, nh * 128, dtype=dtype, device="cuda")
+            kc = torch.zeros(nkv, 1024, 128, dtype=dtype, device="cuda")
+            vc = torch.zeros(nkv, 1024, 128, dtype=dtype, device="cuda")
+            torch.cuda.synchronize()
+            for r0 in (range(0, M, 64) if blocks else [0]):
+                check(lib, run(r0, min(64, M - r0) if blocks else M, splitk, out, q_out, kc, vc))
+            results.append((out, q_out, kc, vc))
+        for what, a, b in zip(("out", "q", "K cache", "V cache"), *results):
+            assert torch.equal(a.view(torch.int16), b.view(torch.int16)), (
+                f"{epi} M={M} splitk={splitk}: {what} of the 256-row launch differs from the 64-row launches in "
+                f"{int((a != b).sum())} elements, max {float((a.float() - b.float()).abs().max()):.3g}")
 
 
 # ----------------------------------------------------------------------------------------------

@@ -70,15 +70,15 @@ def test_w8_gemm_bitwise_equal_to_the_gemm_on_dequantized_weights(lib, epi, dtyp
         rows = 2 * N if epi == "swiglu" else N
         q, scb, wd = quantized(rows, K, N + K, dtype)
         g = torch.Generator(device="cuda").manual_seed(K)
-        X = (torch.randn(64, K, generator=g, device="cuda") * 0.5).to(dtype)
+        X = (torch.randn(256, K, generator=g, device="cuda") * 0.5).to(dtype)  # 256 rows: the prefill launch reads them all
         bias = (torch.randn(N, generator=g, device="cuda") * 0.1).to(dtype) if epi == "store" else None
-        res = torch.randn(64, N, generator=g, device="cuda").to(dtype) if epi == "residual" else None
+        res = torch.randn(256, N, generator=g, device="cuda").to(dtype) if epi == "residual" else None
         torch.cuda.synchronize()
-        for M in (1, 10, 16, 60, 64):
+        for M in (1, 10, 16, 60, 64) + (() if epi == "store" else (65, 200, 256)):  # > 64: the prompt prefill's 256-row launch
             for sk in sorted({1, engine_splitk(rows, K)}):
                 outs = []
                 for w8 in (True, False):
-                    out = res.clone() if res is not None else torch.zeros(64, N, dtype=dtype, device="cuda")
+                    out = res.clone() if res is not None else torch.zeros(256, N, dtype=dtype, device="cuda")
                     torch.cuda.synchronize()
                     rp = C.c_void_p(out.data_ptr()) if res is not None else None
                     bp = C.c_void_p(bias.data_ptr()) if bias is not None else None
@@ -92,8 +92,8 @@ def test_w8_gemm_bitwise_equal_to_the_gemm_on_dequantized_weights(lib, epi, dtyp
                     outs.append(out)
                 a, b = outs
                 assert torch.equal(a.view(torch.int16), b.view(torch.int16)), f"{epi} M={M} N={N} K={K} splitk={sk}"
-                if epi != "residual" and M < 64:
-                    assert float(a[M:].float().abs().max()) == 0.0  # rows beyond M are never written
+                want = res[M:] if res is not None else torch.zeros_like(a[M:])
+                assert torch.equal(a[M:].view(torch.int16), want.view(torch.int16))  # rows beyond M are never written
                 n_cmp += 1
     assert n_cmp >= 10
 
@@ -105,7 +105,8 @@ def test_w8_gemm_rejects_what_it_does_not_run(lib):
     out = torch.zeros(64, 128, dtype=torch.bfloat16, device="cuda")
     p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
     assert lib.eb200_k_gemm_w8(0, 2, p(q), p(scb), p(X), p(out), None, None, 4, 128, 64, 1, None) != 0  # two-matrix SwiGLU
-    assert lib.eb200_k_gemm_w8(0, 0, p(q), p(scb), p(X), p(out), None, None, 65, 128, 64, 1, None) != 0  # M > 64
+    assert lib.eb200_k_gemm_w8(0, 0, p(q), p(scb), p(X), p(out), None, None, 65, 128, 64, 1, None) != 0  # store at 256 rows
+    assert lib.eb200_k_gemm_w8(0, 1, p(q), p(scb), p(X), p(out), p(out), None, 257, 128, 64, 1, None) != 0  # M > 256
     assert lib.eb200_k_gemm_w8(0, 0, p(q), None, p(X), p(out), None, None, 4, 128, 64, 1, None) != 0  # no scales
 
 
