@@ -241,6 +241,30 @@ def correlated_llama3_eagle3(num_layers: int, dtype: torch.dtype, device, draft_
     return tcfg, tW, hcfg, hW
 
 
+def correlated_llama2_eagle1(name: str, num_layers: int, dtype: torch.dtype, device, head_scale: Optional[float] = None,
+                             corrupt_frac: float = 0.25, seed: int = 30):
+    """An EAGLE-1 pair at the width of a named Llama-2 shape ("vicuna-7b", "llama2-13b": MHA, rope theta 1e4, V = 32000) with
+    `num_layers` target layers: a permutation-bigram target + an EAGLE-1 copy head (fc over 2H with bias; the draft reads the
+    target lm_head) whose own embed_tokens has `corrupt_frac` of its rows rotated among themselves, so the draft is wrong after
+    those tokens and accept lengths vary.  head_scale (make_bigram_target_'s, default 0.05, a sharp target): a few tens over H
+    gives a soft one.  The bigram logit is head_scale * <emb(t), final hidden>, below head_scale * H at model width because the
+    random layers add about as much to the residual stream as the embedding carries.  Load the head with load_emb_from_target=False (as from_pretrained
+    does), or the engine embeds with the target's table.  Returns (tcfg, tW, hcfg, hW)."""
+    tcfg = target_config(name)
+    tcfg["num_hidden_layers"] = num_layers
+    hcfg = head_config(name, False)
+    tW = make_target_weights(tcfg, seed, dtype, device=device)
+    make_bigram_target_(tW, tcfg, residual_eps=0.5, **({} if head_scale is None else dict(head_scale=head_scale)))
+    hW = make_copy_head_eagle1_(make_head_weights(hcfg, tW, False, seed + 1, dtype, device=device), tW)
+    if corrupt_frac > 0:
+        E = hW["embed_tokens.weight"]
+        g = torch.Generator()
+        g.manual_seed(seed + 2)
+        idx = torch.randperm(E.shape[0], generator=g)[: max(2, int(E.shape[0] * corrupt_frac))].to(E.device)
+        E[idx] = E[idx.roll(1)]
+    return tcfg, tW, hcfg, hW
+
+
 def draft_vocab_ids(vocab_size: int, draft_vocab_size: int) -> torch.Tensor:
     """Target-vocabulary ids reachable through make_d2t's strided map."""
     return torch.arange(draft_vocab_size, dtype=torch.long) * (vocab_size // draft_vocab_size)

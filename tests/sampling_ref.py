@@ -148,28 +148,32 @@ class _Draw(float):
 
     def __le__(self, other):
         p, lv = float(other), self.level
-        lv["log"].append((float(self), p, lv["keep"]))
+        lv["log"].append((float(self), p, lv["keep"], lv["n"]))
         if not float(self) <= p:
             lv["keep"] *= 1.0 - p  # gtp[xi] = 0; gtp /= gtp.sum(): the next probabilities are relative to what is left
         return float(self) <= p
 
 
-def posterior(lt_nodes: torch.Tensor, thr: torch.Tensor, candidates: torch.Tensor, retrieve: torch.Tensor, uniforms):
+def posterior(lt_nodes: torch.Tensor, thr: torch.Tensor, candidates: torch.Tensor, retrieve: torch.Tensor, uniforms, draws=None):
     """utils.py:375-415 on the kernel's warped rows.
 
     lt_nodes: float64 [T][V] temperature-warped logits of the tree nodes; thr: [T] the stats kernel's thresholds;
     candidates / retrieve: [n_leaf][max_depth] tokens / node ids (-1 padding).  Returns best, accept_length, the bonus
     distribution (float64 [V], zero where ineligible), the number of uniforms the kernel draws (candidates tried + 1 for
-    the bonus), and whether any decision was ambiguous."""
+    the bonus), and whether any decision was ambiguous.  draws: an optional list that receives one (level, accepted) pair
+    per candidate decision, level counted from 0 for each warped row the walk evaluates."""
     masked = torch.where(lt_nodes >= thr.double()[:, None], lt_nodes, torch.full_like(lt_nodes, -math.inf))
-    level = {"log": [], "keep": 1.0}
+    level = {"log": [], "keep": 1.0, "n": -1}
     it = iter(uniforms)
 
-    def warp(row):  # called once per level, before the level's comparisons
+    def warp(row):  # called once per level, before the level's comparisons (and once more for a fresh bonus row)
         level["keep"] = 1.0
+        level["n"] += 1
         return row
 
     best, acc, sample_p = orc.evaluate_posterior_sampling(masked[retrieve.clamp(min=0)], candidates, warp,
                                                           rand=lambda: _Draw(next(it), level))
-    ambiguous = any(abs(u - a) <= AMBIGUOUS_REL * a / max(keep, 1e-30) for u, a, keep in level["log"])
+    if draws is not None:
+        draws.extend((lv, u <= a) for u, a, keep, lv in level["log"])
+    ambiguous = any(abs(u - a) <= AMBIGUOUS_REL * a / max(keep, 1e-30) for u, a, keep, _ in level["log"])
     return int(best), int(acc), sample_p.double(), len(level["log"]) + 1, ambiguous

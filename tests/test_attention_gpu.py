@@ -135,6 +135,7 @@ SWEEP = [
     (BF, 32, 8, 8192, 8192, 10, 65, "straddle", 4.0),
     (BF, 8, 1, 256, 100, 10, 8, "tree", 9.0),
     (FP, 20, 20, 128, 70, 8, 8, "tree", 4.0),
+    (FP, 40, 40, 768, 620, 60, 60, "tree", 4.0),  # Llama-2-13B's verify pass: fp16, 40 query / 40 kv heads
 ]
 
 

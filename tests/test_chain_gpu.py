@@ -29,7 +29,12 @@ CHAIN_GEMM_CASES = [
     # M, N, K   (tiny problems leave most CTAs without a unit; odd tile counts; the benchmark's projection shapes)
     (1, 256, 256), (10, 512, 256), (60, 256, 2048), (64, 1024, 512), (7, 384, 768), (33, 200, 320),
     (60, 4096, 4096), (60, 6144, 4096), (60, 4096, 14336), (10, 32000, 4096), (10, 4096, 12288),
+    # the sampling path's verify lm_head (FIN_STORE_DIRECT, all 60 rows of logits) at Llama-2-13B and Llama-3-8B width, and the
+    # prefill's one-row lm_head at 13B width
+    (60, 32000, 5120), (60, 128256, 4096), (1, 32000, 5120),
 ]
+# 1002 weight tiles: more than the stream-K finish table holds, so the chain kernel refuses FIN_STORE and runs FIN_STORE_DIRECT
+STORE_REFUSED = {(60, 128256, 4096)}
 
 
 @pytest.mark.parametrize("mode", [0, 1])
@@ -43,6 +48,10 @@ def test_chain_gemm_store(lib, M, N, K, dtype, mode):
     want = (X[:M].float() @ W.float().t() + bias.float()).to(dtype)
     out = torch.zeros(64, N, dtype=dtype, device="cuda")
     torch.cuda.synchronize()
+    if mode == 0 and (M, N, K) in STORE_REFUSED:
+        assert lib.eb200_k_chain_gemm(DT[dtype], mode, ptr(W), ptr(X), ptr(out), ptr(bias), None, M, N, K, 1, None) != 0
+        assert "shape not supported" in lib.eb200_last_error().decode()
+        return
     # three launches back to back: the phase counters reset themselves between launches
     check(lib, lib.eb200_k_chain_gemm(DT[dtype], mode, ptr(W), ptr(X), ptr(out), ptr(bias), None, M, N, K, 3, None))
     close(out[:M], want, dtype, f"chain gemm M={M} N={N} K={K} mode={mode}")

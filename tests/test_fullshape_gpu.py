@@ -15,10 +15,10 @@ import torch
 from oracle import eagle_oracle as orc
 from tests.fixtures import report, to_cfg
 from tests.test_e2e_gpu import node_map
+from tests.test_tree_geometry_gpu import frontier_logits_bar
 
 pytestmark = pytest.mark.gpu
 
-ULP_BF16 = 2.0 ** -7
 TREE = dict(total_token=60, depth=6, top_k=10)
 P, NEW = 700, 150
 
@@ -90,21 +90,8 @@ def test_draft_logits_within_1e3_of_the_oracle(pair):
     # low-probability filler whose cumulative scores tie in bf16, so the two implementations may feed DIFFERENT tokens there
     # (torch.topk orders ties arbitrarily) and those rows are not comparable.  Rows are paired by distance and a pair counts as
     # "the same node" when the bulk of the row agrees (median error below 0.05, logits are O(1..200)).
-    d = (got[:, None, :] - want[None, :, :]).abs().median(-1).values
-    used, worst, pairs = set(), 0.0, []
-    for i in range(got.shape[0]):
-        j = min((jj for jj in range(want.shape[0]) if jj not in used), key=lambda jj: float(d[i, jj]))
-        if float(d[i, j]) < 0.05:
-            used.add(j)
-            pairs.append((i, j))
+    pairs, n_bad, n_all, worst = frontier_logits_bar(got, want, torch.bfloat16)
     assert len(pairs) >= 3, f"only {len(pairs)} of {got.shape[0]} frontier rows are fed the same node in both implementations"
-    n_bad, n_all = 0, 0
-    for i, j in pairs:
-        err = (got[i] - want[j]).abs()
-        tol = 1e-3 + ULP_BF16 * want[j].abs()
-        n_bad += int((err > tol).sum())
-        n_all += err.numel()
-        worst = max(worst, float((err / (1e-3 + ULP_BF16 * want[j].abs())).max()))
     report(f"full-shape draft logits ({len(pairs)} comparable frontier rows): {n_bad}/{n_all} elements beyond 1e-3 + 1 ulp; worst error {worst:.2f} x tolerance")
     assert n_bad <= n_all * 1e-3 and worst <= 3.0, f"{n_bad}/{n_all} draft logits beyond 1e-3 + 1 bf16 ulp; worst {worst:.2f}x"
 

@@ -117,21 +117,35 @@ def test_gemm_store(lib, M, N, K, splitk, dtype, simt):
         assert float(out[M:].abs().max()) == 0.0  # rows beyond M are never written
 
 
-@pytest.mark.parametrize("M,N,K,splitk,epi", [
-    (60, 6144, 4096, 4, "qkv"), (60, 4096, 4096, 8, "res"), (60, 14336, 4096, 2, "swiglu"), (60, 4096, 14336, 8, "res"),
-    (60, 128256, 4096, 1, "store"), (10, 32000, 4096, 1, "store"), (10, 6144, 8192, 4, "store"), (8, 4096, 12288, 8, "store"),
+LLAMA3_8B_KV, LLAMA2_7B_KV, LLAMA2_13B_KV = 8, 32, 40
+
+
+@pytest.mark.parametrize("M,N,K,splitk,epi,nkv", [
+    (60, 6144, 4096, 4, "qkv", LLAMA3_8B_KV), (60, 4096, 4096, 8, "res", None), (60, 14336, 4096, 2, "swiglu", None),
+    (60, 4096, 14336, 8, "res", None), (60, 128256, 4096, 1, "store", None), (10, 32000, 4096, 1, "store", None),
+    (10, 6144, 8192, 4, "store", None), (8, 4096, 12288, 8, "store", None),
     # a full 256-row prompt chunk: Llama-3-8B qkv / o / gate_up / down, Llama-3-70B o / down
-    (256, 6144, 4096, 4, "qkv"), (256, 4096, 4096, 4, "res"), (256, 14336, 4096, 1, "swiglu"), (256, 4096, 14336, 4, "res"),
-    (256, 8192, 8192, 2, "res"), (256, 8192, 28672, 2, "res"),
+    (256, 6144, 4096, 4, "qkv", LLAMA3_8B_KV), (256, 4096, 4096, 4, "res", None), (256, 14336, 4096, 1, "swiglu", None),
+    (256, 4096, 14336, 4, "res", None), (256, 8192, 8192, 2, "res", None), (256, 8192, 28672, 2, "res", None),
+    # Vicuna-7B / Llama-2-13B (MHA, I = 11008 / 13824) at the verify pass's 60 rows and a 256-row prompt chunk: qkv, o, gate_up,
+    # down; and the EAGLE-1 head's fc over cat(emb, hidden) with its bias (the draft runs at most 64 rows, so 60 only)
+    (60, 3 * 4096, 4096, 4, "qkv", LLAMA2_7B_KV), (60, 4096, 4096, 8, "res", None), (60, 11008, 4096, 2, "swiglu", None),
+    (60, 4096, 11008, 4, "res", None), (60, 4096, 2 * 4096, 8, "fc", None),
+    (256, 3 * 4096, 4096, 4, "qkv", LLAMA2_7B_KV), (256, 4096, 4096, 4, "res", None), (256, 11008, 4096, 1, "swiglu", None),
+    (256, 4096, 11008, 4, "res", None),
+    (60, 3 * 5120, 5120, 4, "qkv", LLAMA2_13B_KV), (60, 5120, 5120, 8, "res", None), (60, 13824, 5120, 2, "swiglu", None),
+    (60, 5120, 13824, 8, "res", None), (60, 5120, 2 * 5120, 8, "fc", None),
+    (256, 3 * 5120, 5120, 4, "qkv", LLAMA2_13B_KV), (256, 5120, 5120, 4, "res", None), (256, 13824, 5120, 1, "swiglu", None),
+    (256, 5120, 13824, 4, "res", None),
 ])
 @pytest.mark.parametrize("mode", [0, 2])
-def test_gemm_llama3_8b_shapes(lib, M, N, K, splitk, epi, mode):
-    """The projections of the benchmark configuration (BASELINE.json configs[1..2]) at full size, and those of a 256-row
-    prompt chunk of Llama-3-8B and -70B, checked against a float64 reference on sampled output columns (size-independent
-    property: linearity in W rows).  At 256 rows the prefill's epilogues run: gate/up interleaved, and qkv through the
-    QKV + RoPE epilogue with an identity rotation (cos 1, sin 0), which makes it a store into q and the K / V caches (the
-    rotation itself is held to the reference by test_qkv_rope_kv_append)."""
-    dtype = torch.bfloat16
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+def test_gemm_llama3_8b_shapes(lib, M, N, K, splitk, epi, nkv, mode, dtype):
+    """The projections of the benchmark configurations (BASELINE.json: Llama-3-8B, Vicuna-7B, Llama-2-13B) at full size in both
+    model dtypes, and those of a 256-row prompt chunk (Llama-3-70B's o / down too), checked against a float64 reference on
+    sampled output columns (size-independent property: linearity in W rows).  At 256 rows the prefill's epilogues run: gate/up
+    interleaved, and qkv through the QKV + RoPE epilogue with an identity rotation (cos 1, sin 0), which makes it a store into
+    q and the K / V caches (the rotation itself is held to the reference by test_qkv_rope_kv_append)."""
     R = x_rows(M)
     g = torch.Generator(device="cuda").manual_seed(N + K)
     X = (torch.randn(R, K, generator=g, device="cuda") * 0.5).to(dtype)
@@ -145,9 +159,9 @@ def test_gemm_llama3_8b_shapes(lib, M, N, K, splitk, epi, mode):
         if M > 64:
             Wil = interleave64(W, W2)
             torch.cuda.synchronize()
-            check(lib, lib.eb200_k_gemm(0, mode, 5, ptr(Wil), None, ptr(X), ptr(out), None, None, M, N, K, splitk, None))
+            check(lib, lib.eb200_k_gemm(DT[dtype], mode, 5, ptr(Wil), None, ptr(X), ptr(out), None, None, M, N, K, splitk, None))
         else:
-            check(lib, lib.eb200_k_gemm(0, mode, 2, ptr(W), ptr(W2), ptr(X), ptr(out), None, None, M, N, K, splitk, None))
+            check(lib, lib.eb200_k_gemm(DT[dtype], mode, 2, ptr(W), ptr(W2), ptr(X), ptr(out), None, None, M, N, K, splitk, None))
         gate = (X[:M].double() @ W[cols].double().t()).to(dtype)
         up = (X[:M].double() @ W2[cols].double().t()).to(dtype)
         want = F.silu(gate) * up
@@ -156,25 +170,25 @@ def test_gemm_llama3_8b_shapes(lib, M, N, K, splitk, epi, mode):
         assert bool((err <= tol).all()), f"max err {float(err.max())}"
         return
     res = torch.randn(R, N, generator=g, device="cuda").to(dtype) if epi == "res" else None
+    bias = (torch.randn(N, generator=g, device="cuda") * 0.1).to(dtype) if epi == "fc" else None
     torch.cuda.synchronize()
     out = res.clone() if res is not None else torch.zeros(R, N, dtype=dtype, device="cuda")
     torch.cuda.synchronize()
     if epi == "qkv" and M > 64:
-        nkv = 8
-        nh = N // 128 - 2 * nkv  # Llama-3-8B: 32 query heads, 8 kv heads
+        nh = N // 128 - 2 * nkv
         cos = torch.ones(M, 64, dtype=dtype, device="cuda")
         kc = torch.zeros(nkv, M, 128, dtype=dtype, device="cuda")
         vc = torch.zeros(nkv, M, 128, dtype=dtype, device="cuda")
         q_out = torch.zeros(R, nh * 128, dtype=dtype, device="cuda")
         torch.cuda.synchronize()
-        check(lib, lib.eb200_k_qkv_rope(0, mode, ptr(W), ptr(X), ptr(q_out), ptr(kc), ptr(vc), ptr(cos), ptr(torch.zeros_like(cos)), None,
+        check(lib, lib.eb200_k_qkv_rope(DT[dtype], mode, ptr(W), ptr(X), ptr(q_out), ptr(kc), ptr(vc), ptr(cos), ptr(torch.zeros_like(cos)), None,
                                         M, nh, nkv, K, M, 0, splitk, None))
         out = torch.cat((q_out[:M], kc.transpose(0, 1).reshape(M, -1), vc.transpose(0, 1).reshape(M, -1)), dim=1)
     else:
         code = 1 if epi == "res" else 0
-        check(lib, lib.eb200_k_gemm(0, mode, code, ptr(W), None, ptr(X), ptr(out), ptr(out) if res is not None else None, None, M, N, K,
-                                    splitk, None))
-    proj = (X[:M].double() @ W[cols].double().t()).to(dtype)
+        check(lib, lib.eb200_k_gemm(DT[dtype], mode, code, ptr(W), None, ptr(X), ptr(out), ptr(out) if res is not None else None, ptr(bias),
+                                    M, N, K, splitk, None))
+    proj = (X[:M].double() @ W[cols].double().t() + (bias[cols].double() if bias is not None else 0)).to(dtype)
     want = (res[:M][:, cols] + proj) if res is not None else proj
     err = (out[:M][:, cols].float() - want.float()).abs()
     tol = 1e-3 + ULP[dtype] * (proj.float().abs() + want.float().abs())

@@ -92,6 +92,29 @@ def check_tree(dt, ri, tm, tp, tree, what):
     assert sorted(ends) == leaves, f"{what}: retrieve rows end in {sorted(ends)}, the leaves are {leaves}"
 
 
+def frontier_logits_bar(got, want, dtype):
+    """Last-level draft logits [k, V] of the engine (got) against the oracle's (want).  Rows belong to the k frontier nodes; tied
+    low-probability filler may be fed different tokens by the two implementations (torch.topk orders ties arbitrarily), so rows
+    are paired by distance (median error below 0.05) and only rows of the same node are compared, element-wise against
+    1e-3 + one ulp of the model dtype.  Returns (pairs, elements beyond the bar, elements compared, worst error / bar)."""
+    k = got.shape[0]
+    d = (got[:, None, :] - want[None, :, :]).abs().median(-1).values
+    used, pairs = set(), []
+    for i in range(k):
+        j = min((jj for jj in range(want.shape[0]) if jj not in used), key=lambda jj: float(d[i, jj]))
+        if float(d[i, j]) < 0.05:
+            used.add(j)
+            pairs.append((i, j))
+    n_bad, n_all, worst = 0, 0, 0.0
+    for i, j in pairs:
+        err = (got[i] - want[j]).abs()
+        tol = 1e-3 + ULP[dtype] * want[j].abs()
+        n_bad += int((err > tol).sum())
+        n_all += err.numel()
+        worst = max(worst, float((err / tol).max()))
+    return pairs, n_bad, n_all, worst
+
+
 def compare_cycles(m, ref, prompt, tree, what, new_tokens=48, max_length=512, min_shared=None):
     """Whole call, then cycle by cycle against the oracle's log.  Returns (accept lengths, shared verify nodes compared)."""
     ref.cycle_log = []
@@ -189,23 +212,8 @@ def test_last_level_draft_logits_within_1e3_of_the_oracle(tree):
     m.step()
     got = m.debug_read("draft_logits")[:k]
     assert got.shape == want.shape
-    # rows belong to the k frontier nodes of the last level; tied low-probability filler may be fed different tokens by the two
-    # implementations (torch.topk orders ties arbitrarily), so rows are paired by distance and only rows of the same node compared
-    d = (got[:, None, :] - want[None, :, :]).abs().median(-1).values
-    used, pairs = set(), []
-    for i in range(k):
-        j = min((jj for jj in range(k) if jj not in used), key=lambda jj: float(d[i, jj]))
-        if float(d[i, j]) < 0.05:
-            used.add(j)
-            pairs.append((i, j))
+    pairs, n_bad, n_all, worst = frontier_logits_bar(got, want, w[5])
     assert len(pairs) >= 3, f"only {len(pairs)} of {k} frontier rows are fed the same node in both implementations"
-    n_bad, n_all, worst = 0, 0, 0.0
-    for i, j in pairs:
-        err = (got[i] - want[j]).abs()
-        tol = 1e-3 + ULP[w[5]] * want[j].abs()
-        n_bad += int((err > tol).sum())
-        n_all += err.numel()
-        worst = max(worst, float((err / tol).max()))
     report(f"tree geometry {tid(tree)}: last-level draft logits over {(tree['depth']) * k} columns, {len(pairs)} comparable rows, "
            f"{n_bad}/{n_all} beyond 1e-3 + 1 ulp, worst {worst:.2f} x tolerance")
     assert n_bad <= n_all * 1e-3 and worst <= 3.0, f"{n_bad}/{n_all} draft logits beyond 1e-3 + 1 ulp; worst {worst:.2f}x"
