@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libeagle_b200.so")
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 BF16, FP16 = 0, 1
 DT_BF16, DT_FP16, DT_FP32, DT_INT64, DT_BOOL, DT_INT8, DT_UINT8, DT_FP8_E4M3 = 0, 1, 2, 3, 4, 5, 6, 7
 FLAG_SIMT_GEMM, FLAG_NO_GRAPH, FLAG_NO_CHAIN, FLAG_TARGET_INT8 = 1, 2, 4, 8
@@ -93,8 +93,6 @@ SIGNATURES = {
     "eb200_k_gemm_w8": (_I32, [_I32, _I32, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P]),
     "eb200_k_gemm_fp8": (_I32, [_I32, _I32, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P]),
     "eb200_k_gemm_w4": (_I32, [_I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P]),
-    "eb200_k_chain_layer": (_I32, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P, _P,
-                                    _P, _I32, C.c_float, _P]),
     "eb200_k_chain_gemm": (_I32, [_I32, _I32, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P]),
     "eb200_k_gemm_bench": (_I32, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, C.POINTER(C.c_double)]),
     "eb200_k_rmsnorm": (_I32, [_I32, _P, _P, _P, _I32, _I32, C.c_float, _P]),

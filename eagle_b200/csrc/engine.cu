@@ -281,21 +281,17 @@ struct eb200_engine {
   char* tp_win = nullptr;
   size_t tp_win_bytes = 0;
   char* tp_peer[kMaxTp] = {};
-  bool tp_fused = false;        // peers opened: row-parallel projections finish inside the chain launch
+  bool tp_fused = false;        // peers opened: row-parallel projections finish over peer memory (tp_fused.cu), not through NCCL
   long tp_inbox_off = 0, tp_flag_off = 0, tp_ready_off = 0, tp_am_off = 0;
   int* tp_epoch = nullptr;
-  int* tp_ready_base = nullptr;
-  // persistent GEMM chain (mega.cu)
-  int* chain_sync = nullptr;    // [16] self-resetting phase counters
+  // lm_head launch (mega.cu)
+  int* chain_sync = nullptr;    // [2] self-resetting counters
   unsigned long long* chain_timing = nullptr;  // [4] in-kernel %globaltimer accounting (ns sum, launches, scratch)
-  unsigned long long* chain_trace = nullptr;   // EB200_CHAIN_TRACE=<file>: phase stamps of the verify pass' layer-5 chain launch
   double chain_bytes_cycle = 0;  // algorithmic bytes of the chain launches captured in the cycle graph
   double chain_bytes_pending = 0;
   float* tile_val = nullptr;    // [lm_head tiles][64] per-tile row maxima of the fused arg-max
   int* tile_idx = nullptr;
-  bool chain_target = false;    // the target's layer segments run as chain launches
-  bool chain_head = false;      // ... including the lm_head (fused arg-max / direct store)
-  bool chain_draft = false;     // the draft head's layer tail + lm_head run as one chain launch per pass
+  bool chain_head = false;      // the target lm_head runs as one mega.cu launch (fused arg-max / direct store)
   bool fused_e3_input = true;   // EAGLE-3 draft input (gather + two RMSNorms + concat) as one launch
   std::map<const void*, CUtensorMap> kv_maps;  // TMA descriptors of the K/V cache planes (attention.cu), built on first use
 };
@@ -504,7 +500,6 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
       TRY(make_tmap(&e->xn.tm16, e->dtype, e->xn.p, 64, H, 16));
       TRY(make_tmap(&e->xn.tm64, e->dtype, e->xn.p, 64, H, 64));
       TRY(dalloc(e, reinterpret_cast<void**>(&e->tp_epoch), 64));
-      TRY(dalloc(e, reinterpret_cast<void**>(&e->tp_ready_base), 64));
     } else {
       TRY(dalloc(e, &e->x, static_cast<size_t>(e->act_rows) * H * 2));
       TRY(dalloc(e, &e->feat, static_cast<size_t>(64) * e->F * 2));
@@ -530,7 +525,7 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
     e->ws_bytes = static_cast<size_t>(96) << 20;
     TRY(dalloc(e, reinterpret_cast<void**>(&e->ws), e->ws_bytes, false));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->counters), 8192 * sizeof(int)));
-    TRY(dalloc(e, reinterpret_cast<void**>(&e->chain_sync), 16 * sizeof(int)));
+    TRY(dalloc(e, reinterpret_cast<void**>(&e->chain_sync), 2 * sizeof(int)));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->chain_timing), 4 * sizeof(unsigned long long)));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->tile_val), static_cast<size_t>((e->V_l + 127) / 128) * 64 * sizeof(float)));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->tile_idx), static_cast<size_t>((e->V_l + 127) / 128) * 64 * sizeof(int)));
@@ -572,7 +567,6 @@ extern "C" int eb200_create(const eb200_config* cfg, eb200_engine** out) {
     TRY(dalloc(e, reinterpret_cast<void**>(&e->st_src), kStaticMaxNodes * sizeof(int)));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->st_lmask), kStaticMaxNodes * 2 * sizeof(uint64_t)));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->ss_tokens), (kStaticMaxNodes + 1) * 32 * sizeof(int)));
-    if (getenv("EB200_CHAIN_TRACE")) TRY(dalloc(e, reinterpret_cast<void**>(&e->chain_trace), 256 * 32 * sizeof(unsigned long long)));
     if (getenv("EB200_ATTN_TRACE")) TRY(dalloc(e, reinterpret_cast<void**>(&e->attn_trace), 8192 * 16 * sizeof(unsigned long long)));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->ids_dev), static_cast<size_t>(c.max_length + 128) * 8));
     TRY(dalloc(e, reinterpret_cast<void**>(&e->out_ids_dev), static_cast<size_t>(c.max_length + 128) * 8));
@@ -609,20 +603,6 @@ extern "C" void eb200_destroy(eb200_engine* e) {
           if (!h[c * 16]) continue;
           fprintf(f, "%zu", c);
           for (int j = 0; j < 16; ++j) fprintf(f, " %llu", h[c * 16 + j]);
-          fprintf(f, "\n");
-        }
-        fclose(f);
-      }
-    }
-  }
-  if (e->chain_trace) {
-    std::vector<unsigned long long> h(256 * 32);
-    if (cudaMemcpy(h.data(), e->chain_trace, h.size() * 8, cudaMemcpyDeviceToHost) == cudaSuccess) {
-      if (FILE* f = fopen(getenv("EB200_CHAIN_TRACE"), "w")) {
-        for (size_t c = 0; c < 256; ++c) {
-          if (!h[c * 32]) continue;
-          fprintf(f, "%zu", c);
-          for (int j = 0; j < 32; ++j) fprintf(f, " %llu", h[c * 32 + j]);
           fprintf(f, "\n");
         }
         fclose(f);
@@ -1020,10 +1000,8 @@ extern "C" int eb200_finalize(eb200_engine* e) {
                       : (e->c.flags & EB200_FLAG_TARGET_FP8) ? "FP8 target weights (EB200_FLAG_TARGET_FP8)"
                                                              : "4-bit target weights (EB200_FLAG_TARGET_NF4 / _FP4)";
     const char* what = nullptr;
-    const char* chain = getenv("EB200_CHAIN");
     if (e->c.tp_size > 1) what = "tensor parallelism (tp_size > 1)";
     else if (e->c.flags & EB200_FLAG_SIMT_GEMM) what = "EB200_FLAG_SIMT_GEMM";
-    else if (chain && atoi(chain) == 1) what = "EB200_CHAIN=1 (persistent layer-segment launches)";
     if (what)
       return fail("%s are not supported with %s; they run on one GPU with the default cluster split-K GEMM", fmt, what);
   }
@@ -1058,26 +1036,11 @@ extern "C" int eb200_finalize(eb200_engine* e) {
     if (e->d2t && !e->d2t_loaded) return fail("head d2t missing (draft_vocab_size != vocab_size)");
   }
   {
-    // Persistent chain launches (mega.cu).  The layer segment as ONE launch is slower than the per-projection cluster split-K
-    // kernels (its global-memory split-K reduction is bounded by the LSU path of the finishing SMs), so on one GPU only the
-    // lm_head runs as a (single-phase, reduction-free) chain launch with the fused arg-max (no 15 MB logits round trip).
-    // Under tensor parallelism the chain segment is slower as well, so the peer-window exchange runs as its own kernel behind
-    // the per-projection GEMMs (tp_fused.cu) and the chain segment stays opt-in.
-    //   EB200_CHAIN=0 : never;  EB200_CHAIN=1 : layer segments as chain launches (A/B);  EB200_CHAIN_DRAFT=1 : draft head tail too
-    const char* env = getenv("EB200_CHAIN");
-    const int mode = env ? atoi(env) : -1;  // -1 = default policy
-    const bool allowed = mode != 0 && !(e->c.flags & (EB200_FLAG_SIMT_GEMM | EB200_FLAG_NO_CHAIN));
-    const Layer& l0 = e->tl[0];
-    const bool shapes_ok = e->ws_bytes >= chain_ws_bytes(64) && chain_phase_ok(l0.o.N, l0.o.K, FIN_RESID_NORM) &&
-                           chain_phase_ok(l0.gu.N, l0.gu.K, FIN_SWIGLU_IL) && chain_phase_ok(l0.down.N, l0.down.K, FIN_RESID_NORM) &&
-                           chain_phase_ok(l0.qkv.N, l0.qkv.K, FIN_QKV_ROPE);
-    e->chain_target = allowed && shapes_ok && mode == 1 && (e->c.tp_size == 1 || e->tp_fused);
-    e->chain_head = allowed && e->ws_bytes >= chain_ws_bytes(64) && (e->c.tp_size == 1 || e->tp_fused) &&
-                    chain_phase_ok(e->t_head.N, e->t_head.K, FIN_ARGMAX);
-    const Layer& h0 = e->hl[0];
-    const char* denv = getenv("EB200_CHAIN_DRAFT");
-    e->chain_draft = allowed && denv && atoi(denv) == 1 && e->ws_bytes >= chain_ws_bytes(64) && chain_phase_ok(h0.o.N, h0.o.K, FIN_RESID_NORM) &&
-                     chain_phase_ok(h0.gu.N, h0.gu.K, FIN_SWIGLU_IL) && chain_phase_ok(h0.down.N, h0.down.K, FIN_RESID_NORM);
+    // The target lm_head runs as one launch of whole vocabulary tiles per CTA (mega.cu) with the arg-max fused (no 15 MB logits
+    // round trip).  It needs the peer windows under tensor parallelism (vocabulary-parallel arg-max exchange); without them, and
+    // with EB200_FLAG_SIMT_GEMM / EB200_FLAG_NO_CHAIN, the lm_head is a GEMM launch followed by vocab_argmax.
+    e->chain_head = !(e->c.flags & (EB200_FLAG_SIMT_GEMM | EB200_FLAG_NO_CHAIN)) && (e->c.tp_size == 1 || e->tp_fused) &&
+                    chain_phase_ok(e->t_head.N, e->t_head.K);
     const char* fenv = getenv("EB200_FUSED_E3_INPUT");
     e->fused_e3_input = !(fenv && atoi(fenv) == 0);
   }
@@ -1352,7 +1315,7 @@ static int gemm_partial_f32(eb200_engine* e, const RowCtx& cx, const Linear& W, 
 }
 static int tp_allreduce_f32(eb200_engine* e, float* buf, size_t count);
 static int tp_allgather_u32(eb200_engine* e, const void* send, void* recv, size_t count);
-static void chain_fill_tp(eb200_engine* e, ChainArgs& a);
+static void chain_fill_tp(eb200_engine* e, ChainTP& tp);
 // x += W . X  for a row-parallel projection (o_proj, down_proj).  Single GPU: fused residual epilogue.  Tensor parallel: every
 // rank produces an unrounded fp32 partial over its slice of the reduction dim; then either
 //   * NVLink peer windows (default): ONE kernel pushes the partial rows to their owners, reduces them in rank order, applies the
@@ -1367,10 +1330,7 @@ static int row_parallel_residual(eb200_engine* e, const RowCtx& cx, const Linear
   if (e->tp_fused && cx.rows_idx < 0) {
     TpResidParams p;
     memset(&p, 0, sizeof(p));
-    ChainArgs tmp;
-    memset(&tmp, 0, sizeof(tmp));
-    chain_fill_tp(e, tmp);
-    p.tp = tmp.tp;
+    chain_fill_tp(e, p.tp);
     p.partial = e->f32buf;
     p.ld_partial = H;
     p.N = H;
@@ -1609,7 +1569,8 @@ extern "C" int eb200_tp_init(eb200_engine* e, const void* id128) {
   return 0;
 }
 // Peer windows: every rank exports the CUDA IPC handle of its window; after the launcher has exchanged them, each rank maps the
-// others' windows.  From then on the row-parallel projections finish inside the chain launch (ChainTP) instead of through NCCL.
+// others' windows.  From then on the row-parallel projections finish over peer memory (tp_fused.cu) instead of through NCCL, and
+// the lm_head's vocabulary-parallel arg-max exchanges its (value, index) pairs through the same windows.
 extern "C" int eb200_tp_ipc_handle(eb200_engine* e, void* out64) {
   if (!e || !out64) return fail("null argument");
   if (e->c.tp_size <= 1 || !e->tp_win) return fail("eb200_tp_ipc_handle: engine is not tensor parallel");
@@ -1683,143 +1644,22 @@ enum HeadMode : int { HEAD_NONE = 0, HEAD_ARGMAX = 1, HEAD_LOGITS = 2 };
 static bool is_tap_layer(const eb200_engine* e, int i) { return i == e->L - 3 || i == e->L / 2 || i == 2; }
 static int vocab_argmax(eb200_engine* e, int rows);
 
-// finish items per activation row: spread the row-wise finish over the CTAs that are not needed for other rows
-static int chain_chunks(int passes, int rows) {
-  const int G = std::max(1, chain_grid());
-  return std::max(1, std::min(passes, G / std::max(1, rows)));
-}
-static void chain_phase_gemm(ChainArgs& a, ChainMaps& m, int p, const RowCtx& cx, const Linear& W, const ActBuf& X) {
-  a.ph[p].N = W.N;
-  a.ph[p].K = W.K;
-  m.w[p] = W.tm;
-  m.x[p] = cx.mpad == 16 ? X.tm16 : X.tm64;
-}
-
-static void chain_fill_tp(eb200_engine* e, ChainArgs& a) {
+static void chain_fill_tp(eb200_engine* e, ChainTP& tp) {
   if (e->c.tp_size <= 1) return;
-  a.tp.size = e->c.tp_size;
-  a.tp.rank = e->c.tp_rank;
-  for (int r = 0; r < e->c.tp_size; ++r) a.tp.win[r] = e->tp_peer[r];
-  a.tp.inbox_off = e->tp_inbox_off;
-  a.tp.ld_inbox = e->H;
-  a.tp.flag_off = e->tp_flag_off;
-  a.tp.ready_off = e->tp_ready_off;
-  a.tp.am_off = e->tp_am_off;
-  a.tp.epoch = e->tp_epoch;
-  a.tp.ready_base = e->tp_ready_base;
-}
-static void chain_head_phase(eb200_engine* e, ChainArgs& a, ChainMaps& m, int p, const RowCtx& cx, int head_mode) {
-  chain_phase_gemm(a, m, p, cx, e->t_head, e->xn);
-  ChainPhase& h = a.ph[p];
-  h.chunks = 1;
-  if (head_mode == HEAD_ARGMAX) {
-    h.fin = FIN_ARGMAX;
-    h.tile_val = e->tile_val;
-    h.tile_idx = e->tile_idx;
-    h.out_idx = e->node_argmax;
-    if (e->c.tp_size > 1) {  // vocabulary-parallel shard: only the real rows compete, indices are global
-      h.idx_offset = e->c.tp_rank * e->V_l;
-      h.N = std::max(0, std::min(e->V_l, e->V - h.idx_offset));
-    }
-  } else {
-    h.fin = FIN_STORE_DIRECT;
-    h.out = e->logits;
-    h.ld_out = e->V_l;
-  }
-}
-// One chain launch = o_proj(+residual, RMSNorm) -> gate/up(SwiGLU) -> down_proj(+residual, RMSNorm) -> the NEXT block's
-// qkv(+RoPE, KV append) or, after the last layer, the lm_head (fused arg-max, or logits for the sampling path).
-static int target_segment_chain(eb200_engine* e, const RowCtx& cx, int i, void* feat_dst, int* slot, int head_mode) {
-  const int H = e->H, L = e->L;
-  Layer& l = e->tl[i];
-  ChainArgs a;
-  ChainMaps m;
-  memset(&a, 0, sizeof(a));
-  memset(&m, 0, sizeof(m));
-  a.m_rows = cx.rows;
-  a.m_idx = cx.rows_idx;
-  a.st = e->st;
-  a.ws = e->ws;
-  a.sync = e->chain_sync;
-  a.timing = e->chain_timing;
-  chain_fill_tp(e, a);
-  double bytes = 0;
-  int p = 0;
-  // o_proj: x += attn . Wo^T ; xn = post_attention_layernorm(x)      (modeling_llama_kv.py:838-845, :128-132)
-  chain_phase_gemm(a, m, p, cx, l.o, e->attn);
-  a.ph[p].fin = FIN_RESID_NORM;
-  a.ph[p].chunks = 1;
-  a.ph[p].x = e->x;
-  a.ph[p].ld_x = H;
-  a.ph[p].norm_w = l.ln2;
-  a.ph[p].xn = e->xn.p;
-  a.ph[p].ld_xn = H;
-  a.ph[p].eps = e->c.rms_norm_eps;
-  bytes += static_cast<double>(l.o.N) * l.o.K * 2;
-  ++p;
-  // gate/up + SwiGLU (modeling_llama_kv.py:501-535)
-  chain_phase_gemm(a, m, p, cx, l.gu, e->xn);
-  a.ph[p].fin = FIN_SWIGLU_IL;
-  a.ph[p].chunks = chain_chunks((e->I_l + 511) / 512, cx.rows);
-  a.ph[p].out = e->act.p;
-  a.ph[p].ld_out = e->I_l;
-  a.ph[p].silu_lut = silu_lut(e->dtype, e->stream);
-  if (!a.ph[p].silu_lut) return fail("SiLU table not ready (first use inside stream capture)");
-  bytes += static_cast<double>(l.gu.N) * l.gu.K * 2;
-  ++p;
-  // down_proj: x += act . Wd^T ; xn = the next block's input_layernorm(x) (or the final norm)
-  chain_phase_gemm(a, m, p, cx, l.down, e->act);
-  a.ph[p].fin = FIN_RESID_NORM;
-  a.ph[p].chunks = 1;
-  a.ph[p].x = e->x;
-  a.ph[p].ld_x = H;
-  if (e->c.eagle3 && feat_dst && i + 1 < L && is_tap_layer(e, i + 1)) {  // hidden state entering layer i+1 (utils.py:248-252)
-    a.ph[p].tap = reinterpret_cast<char*>(feat_dst) + static_cast<size_t>(*slot) * H * 2;
-    a.ph[p].ld_tap = e->F;
-    ++*slot;
-  }
-  a.ph[p].norm_w = (i + 1 < L) ? e->tl[i + 1].ln1 : e->t_norm;
-  a.ph[p].xn = e->xn.p;
-  a.ph[p].ld_xn = H;
-  a.ph[p].eps = e->c.rms_norm_eps;
-  bytes += static_cast<double>(l.down.N) * l.down.K * 2;
-  ++p;
-  if (i + 1 < L) {
-    Layer& nl = e->tl[i + 1];
-    chain_phase_gemm(a, m, p, cx, nl.qkv, e->xn);
-    ChainPhase& q = a.ph[p];
-    q.fin = FIN_QKV_ROPE;
-    q.chunks = chain_chunks((e->nh_l + 2 * e->nkv_l + 7) / 8, cx.rows);
-    q.q_out = e->q;
-    q.k_cache = kv_plane(e->t_kv, i + 1, 0, e->nkv_l, e->cap);
-    q.v_cache = kv_plane(e->t_kv, i + 1, 1, e->nkv_l, e->cap);
-    q.kv_cap = e->cap;
-    q.n_q_heads = e->nh_l;
-    q.n_kv_heads = e->nkv_l;
-    q.rope_cos = e->t_cos;
-    q.rope_sin = e->t_sin;
-    q.pos_base = cx.pos_base;
-    q.pos_arr = cx.pos_arr;
-    q.pos_mstride = cx.pos_mstride;
-    q.kv_base = cx.kv_base;
-    bytes += static_cast<double>(nl.qkv.N) * nl.qkv.K * 2;
-    ++p;
-  } else if (head_mode != HEAD_NONE && e->chain_head) {
-    chain_head_phase(e, a, m, p, cx, head_mode);
-    bytes += static_cast<double>(e->t_head.N) * e->t_head.K * 2;
-    ++p;
-  }
-  a.n_phases = p;
-  if (e->chain_trace && e->in_verify && i == std::min(5, L - 2)) a.trace = e->chain_trace;
-  if (skip_kernel("chain")) return 0;
-  ProfScope ps(e, 0, bytes, "gemm_chain");
-  CKL(launch_gemm_chain(e->dtype, cx.mpad, m, a, e->stream));
-  e->stats.chain_bytes += bytes;
-  return 0;
+  tp.size = e->c.tp_size;
+  tp.rank = e->c.tp_rank;
+  for (int r = 0; r < e->c.tp_size; ++r) tp.win[r] = e->tp_peer[r];
+  tp.inbox_off = e->tp_inbox_off;
+  tp.ld_inbox = e->H;
+  tp.flag_off = e->tp_flag_off;
+  tp.ready_off = e->tp_ready_off;
+  tp.am_off = e->tp_am_off;
+  tp.epoch = e->tp_epoch;
 }
 
-// lm_head over the rows in e->xn (ea_model.py:190): one reduction-free chain launch (whole 128-row vocabulary tiles per CTA,
-// per-row arg-max straight from the staged accumulator tile, merged per row) or, for the sampling path, the logits of this rank's shard.
+// lm_head over the rows in e->xn (ea_model.py:190): one launch of whole 128-row vocabulary tiles per CTA (mega.cu), with the
+// per-row arg-max taken straight from the staged accumulator tile and merged per row or, for the sampling path, the logits of
+// this rank's shard.
 static int target_head(eb200_engine* e, const RowCtx& cx, int head_mode) {
   if (head_mode == HEAD_NONE) return 0;
   if (!e->chain_head) {
@@ -1834,12 +1674,28 @@ static int target_head(eb200_engine* e, const RowCtx& cx, int head_mode) {
   a.m_rows = cx.rows;
   a.m_idx = cx.rows_idx;
   a.st = e->st;
-  a.ws = e->ws;
   a.sync = e->chain_sync;
   a.timing = e->chain_timing;
-  chain_fill_tp(e, a);
-  chain_head_phase(e, a, m, 0, cx, head_mode);
-  a.n_phases = 1;
+  chain_fill_tp(e, a.tp);
+  ChainPhase& h = a.ph;
+  h.N = e->t_head.N;
+  h.K = e->t_head.K;
+  m.w = e->t_head.tm;
+  m.x = cx.mpad == 16 ? e->xn.tm16 : e->xn.tm64;
+  if (head_mode == HEAD_ARGMAX) {
+    h.fin = FIN_ARGMAX;
+    h.tile_val = e->tile_val;
+    h.tile_idx = e->tile_idx;
+    h.out_idx = e->node_argmax;
+    if (e->c.tp_size > 1) {  // vocabulary-parallel shard: only the real rows compete, indices are global
+      h.idx_offset = e->c.tp_rank * e->V_l;
+      h.N = std::max(0, std::min(e->V_l, e->V - h.idx_offset));
+    }
+  } else {
+    h.fin = FIN_STORE_DIRECT;
+    h.out = e->logits;
+    h.ld_out = e->V_l;
+  }
   const double bytes = static_cast<double>(e->t_head.N) * e->t_head.K * 2;
   if (skip_kernel("chain")) return 0;
   ProfScope ps(e, 0, bytes, "gemm_chain_head");
@@ -1857,26 +1713,6 @@ static int target_forward(eb200_engine* e, const RowCtx& cx, const int64_t* ids6
   const float eps = e->c.rms_norm_eps;
   TRY(gather(e, e->t_embed, H, ids64, ids32, e->x, H, 0, H, cx.rows));
   int slot = 0;
-  if (e->chain_target) {
-    // lead-in (embedding -> first block's norm + qkv) as single kernels, then per block: attention + ONE chain launch
-    if (e->c.eagle3 && feat_dst && is_tap_layer(e, 0)) {
-      TRY(gather(e, e->x, H, nullptr, e->ident, feat_dst, e->F, slot * H, H, cx.rows));
-      ++slot;
-    }
-    TRY(rmsnorm(e, e->x, H, nullptr, nullptr, e->tl[0].ln1, e->xn.p, H, 0, H, eps, cx.rows));
-    TRY(gemm_qkv(e, cx, e->tl[0].qkv, e->xn, e->q, kv_plane(e->t_kv, 0, 0, e->nkv_l, e->cap), kv_plane(e->t_kv, 0, 1, e->nkv_l, e->cap), e->cap,
-                 e->nh_l, e->nkv_l, e->t_cos, e->t_sin));
-    for (int i = 0; i < L; ++i) {
-      void* kc = kv_plane(e->t_kv, i, 0, e->nkv_l, e->cap);
-      void* vc = kv_plane(e->t_kv, i, 1, e->nkv_l, e->cap);
-      const L2Prefetch pf_o = l2_plan(e, e->tl[i].o, cx.mpad, 0, static_cast<double>(e->l2_bytes));  // the chain's first phase
-      TRY(attention(e, cx, e->q, kc, vc, e->attn.p, e->cap, e->nh_l, e->nkv_l, &pf_o));
-      TRY(target_segment_chain(e, cx, i, feat_dst, &slot, head_mode));
-    }
-    if (!e->c.eagle3 && feat_dst) TRY(gather(e, e->xn.p, H, nullptr, e->ident, feat_dst, e->F, 0, H, cx.rows));
-    if (!e->chain_head) TRY(target_head(e, cx, head_mode));  // else: already the last phase of the last segment
-    return 0;
-  }
   bool have_xn = false;   // xn already holds this layer's input_layernorm(x) (written by the previous down_proj's fused TP kernel)
   bool tap_done = false;  // ... and the EAGLE-3 tap of this layer was written there too
   // L2 prefetch: every GEMM's producers fetch the leading weight tiles of the next GEMM after their last load, and the latency-bound
@@ -1922,78 +1758,6 @@ static int target_forward(eb200_engine* e, const RowCtx& cx, const int64_t* ids6
   return 0;
 }
 
-// Tail of one draft decoder layer as ONE chain launch: o_proj(+residual, post-attention norm) -> gate/up(SwiGLU) ->
-// down_proj(+residual [, next norm]) [-> lm_head over all rows when it is the last layer].
-static int draft_segment_chain(eb200_engine* e, const RowCtx& cx, int i) {
-  const int Hh = e->Hh;
-  const bool last = (i == e->hL - 1);
-  Layer& l = e->hl[i];
-  ChainArgs a;
-  ChainMaps m;
-  memset(&a, 0, sizeof(a));
-  memset(&m, 0, sizeof(m));
-  a.m_rows = cx.rows;
-  a.m_idx = cx.rows_idx;
-  a.st = e->st;
-  a.ws = e->ws;
-  a.sync = e->chain_sync;
-  a.timing = e->chain_timing;
-  double bytes = 0;
-  int p = 0;
-  chain_phase_gemm(a, m, p, cx, l.o, e->d_attn);  // h2 = h + o_proj(attn); xn = post_attention_layernorm(h2)   (cnets.py:432-441)
-  a.ph[p].fin = FIN_RESID_NORM;
-  a.ph[p].chunks = 1;
-  a.ph[p].res = e->d_h.p;
-  a.ph[p].ld_res = Hh;
-  a.ph[p].x = e->d_h2;
-  a.ph[p].ld_x = Hh;
-  a.ph[p].norm_w = l.ln2;
-  a.ph[p].xn = e->d_xn.p;
-  a.ph[p].ld_xn = Hh;
-  a.ph[p].eps = e->c.head_rms_norm_eps;
-  bytes += static_cast<double>(l.o.N) * l.o.K * 2;
-  ++p;
-  chain_phase_gemm(a, m, p, cx, l.gu, e->d_xn);
-  a.ph[p].fin = FIN_SWIGLU_IL;
-  a.ph[p].chunks = chain_chunks((e->Ih + 511) / 512, cx.rows);
-  a.ph[p].out = e->d_act.p;
-  a.ph[p].ld_out = e->Ih;
-  a.ph[p].silu_lut = silu_lut(e->dtype, e->stream);
-  if (!a.ph[p].silu_lut) return fail("SiLU table not ready (first use inside stream capture)");
-  bytes += static_cast<double>(l.gu.N) * l.gu.K * 2;
-  ++p;
-  chain_phase_gemm(a, m, p, cx, l.down, e->d_act);  // out = h2 + mlp(xn)
-  a.ph[p].fin = FIN_RESID_NORM;
-  a.ph[p].chunks = 1;
-  a.ph[p].res = e->d_h2;
-  a.ph[p].ld_res = Hh;
-  a.ph[p].x = last ? e->d_out.p : e->d_h.p;
-  a.ph[p].ld_x = Hh;
-  if (e->c.eagle3) a.ph[p].norm_w = e->h_norm;  // lm_head(norm(out))  cnets.py:700, :734
-  else if (!last) a.ph[p].norm_w = e->hl[i + 1].ln1;
-  a.ph[p].xn = e->d_xn.p;
-  a.ph[p].ld_xn = Hh;
-  a.ph[p].eps = e->c.head_rms_norm_eps;
-  bytes += static_cast<double>(l.down.N) * l.down.K * 2;
-  ++p;
-  if (last) {
-    const Linear& head = e->c.eagle3 ? e->h_head : (e->t_head_full.w ? e->t_head_full : e->t_head);
-    chain_phase_gemm(a, m, p, cx, head, e->c.eagle3 ? e->d_xn : e->d_out);
-    a.ph[p].fin = chain_phase_ok(head.N, head.K, FIN_STORE) ? FIN_STORE : FIN_STORE_DIRECT;
-    a.ph[p].chunks = a.ph[p].fin == FIN_STORE ? chain_chunks((head.N + 511) / 512, cx.rows) : 1;
-    a.ph[p].out = e->d_logits;
-    a.ph[p].ld_out = e->Vd;
-    bytes += static_cast<double>(head.N) * head.K * 2;
-    ++p;
-  }
-  a.n_phases = p;
-  if (skip_kernel("chain")) return 0;
-  ProfScope ps(e, 0, bytes, "gemm_chain_draft");
-  CKL(launch_gemm_chain(e->dtype, cx.mpad, m, a, e->stream));
-  e->stats.chain_bytes += bytes;
-  return 0;
-}
-
 // Draft head forward over <= 64 rows.  first_pass: the rows' features are in e->d_feat (EAGLE-3: 3H taps -> fc).  Tree levels
 // (src_rows != nullptr): the hidden input of row m is row src_rows[m] of the previous pass' output e->d_out (cnets.py:716,
 // :747).  Ends with the draft logits of all rows in e->d_logits.
@@ -2018,11 +1782,10 @@ static int draft_forward(eb200_engine* e, const RowCtx& cx, const int64_t* ids64
     }
     void* kc = kv_plane(e->d_kv, 0, 0, e->hnkv, e->dcap);
     void* vc = kv_plane(e->d_kv, 0, 1, e->hnkv, e->dcap);
-    const L2Prefetch pf_o = l2_plan(e, l.o, cx.mpad, 0, e->chain_draft ? 0 : pf_tail_bytes());
+    const L2Prefetch pf_o = l2_plan(e, l.o, cx.mpad, 0, pf_tail_bytes());
     TRY(gemm_qkv(e, cx, l.qkv, e->d_cat, e->d_q, kc, vc, e->dcap, e->hnh, e->hnkv, e->h_cos, e->h_sin, &pf_o));
     const L2Prefetch pf_o_rest = l2_plan_rest(e, l.o, cx.mpad, pf_o);
     TRY(attention(e, cx, e->d_q, kc, vc, e->d_attn.p, e->dcap, e->hnh, e->hnkv, &pf_o_rest));
-    if (e->chain_draft) return draft_segment_chain(e, cx, 0);
     const L2Prefetch pf_gu = l2_plan(e, l.gu, cx.mpad, 0, pf_tail_bytes());
     TRY(gemm_residual(e, cx, l.o, e->d_attn, e->d_h.p, e->d_h2, Hh, &pf_gu));
     const L2Prefetch pf_gu_rest = l2_plan(e, l.gu, cx.mpad, pf_gu.j1, pf_norm_bytes());
@@ -2047,25 +1810,20 @@ static int draft_forward(eb200_engine* e, const RowCtx& cx, const int64_t* ids64
     Layer& l = e->hl[i];
     const ActBuf* xin = &e->d_h;
     if (i > 0) {
-      // chain mode: the previous layer's down_proj finish already produced input_layernorm(h) in d_xn
-      if (!e->chain_draft) TRY(rmsnorm(e, e->d_h.p, Hh, nullptr, nullptr, l.ln1, e->d_xn.p, Hh, 0, Hh, eps, cx.rows));
+      TRY(rmsnorm(e, e->d_h.p, Hh, nullptr, nullptr, l.ln1, e->d_xn.p, Hh, 0, Hh, eps, cx.rows));
       xin = &e->d_xn;
     }
     void* kc = kv_plane(e->d_kv, i, 0, e->hnkv, e->dcap);
     void* vc = kv_plane(e->d_kv, i, 1, e->hnkv, e->dcap);
     TRY(gemm_qkv(e, cx, l.qkv, *xin, e->d_q, kc, vc, e->dcap, e->hnh, e->hnkv, e->h_cos, e->h_sin));
     TRY(attention(e, cx, e->d_q, kc, vc, e->d_attn.p, e->dcap, e->hnh, e->hnkv));
-    if (e->chain_draft) {
-      TRY(draft_segment_chain(e, cx, i));
-      continue;
-    }
     TRY(gemm_residual(e, cx, l.o, e->d_attn, e->d_h.p, e->d_h2, Hh));
     TRY(rmsnorm(e, e->d_h2, Hh, nullptr, nullptr, l.ln2, e->d_xn.p, Hh, 0, Hh, eps, cx.rows));
     TRY(gemm_swiglu(e, cx, l.gu, e->d_xn, e->d_act.p, e->Ih));
     void* dst = (i == e->hL - 1) ? e->d_out.p : e->d_h.p;
     TRY(gemm_residual(e, cx, l.down, e->d_act, e->d_h2, dst, Hh));
   }
-  if (!e->chain_draft) TRY(gemm_store(e, cx, e->t_head_full.w ? e->t_head_full : e->t_head, e->d_out, e->d_logits, e->Vd, nullptr));
+  TRY(gemm_store(e, cx, e->t_head_full.w ? e->t_head_full : e->t_head, e->d_out, e->d_logits, e->Vd, nullptr));
   return 0;
 }
 
@@ -2202,7 +1960,7 @@ static int target_prefill(eb200_engine* e, const int64_t* prompt, int P, int* fi
   int last_rows = 0;
   // 256 prompt rows per pass where the activation buffers allow it (one GPU, wgmma path): the weights are streamed
   // ceil(P / 256) times instead of ceil(P / 64) times (utils.py:232-254 runs the whole prompt in one forward)
-  const int chunk = (e->act_rows >= 256 && !e->chain_target) ? 256 : 64;
+  const int chunk = e->act_rows >= 256 ? 256 : 64;
   for (int base = 0; base < P; base += chunk) {
     const int rows = std::min(chunk, P - base);
     TRY(set_state(e, S_TMP0, base));
@@ -3057,102 +2815,33 @@ extern "C" int eb200_k_gemm_fp8(int32_t dtype, int32_t epilogue, const void* Wq,
   return rc;
 }
 
-// One decoder-layer segment through the persistent chain kernel (mega.cu), on caller tensors (all DEVICE pointers):
-//   x += attn . Wo^T ; xn = ln2 * norm(x) ; act = swiglu(xn . Wgu^T) ; x += act . Wd^T ; xn = ln1n * norm(x) ;
-//   q / K-cache / V-cache rows <- rope(xn . Wqkv^T)                         (n_phases = 4; 3 stops before the qkv)
-// Wgu is the [2I, H] matrix with gate/up interleaved in 64-row groups.  attn/xn/act are [64][*] buffers (rows >= M ignored).
-extern "C" int eb200_k_chain_layer(int32_t dtype, int32_t M, int32_t H, int32_t I, int32_t n_heads, int32_t n_kv_heads, int32_t n_phases,
-                                   const void* Wo, const void* Wgu, const void* Wdown, const void* Wqkv, const void* ln2, const void* ln1n,
-                                   const void* attn, void* x, void* xn, void* act, void* tap, void* q_out, void* k_cache, void* v_cache,
-                                   int64_t kv_cap, const void* cosp, const void* sinp, const int32_t* pos, int32_t kv_base, float eps,
-                                   void* stream) {
-  if (M < 1 || M > 64 || n_phases < 1 || n_phases > 4) return fail("eb200_k_chain_layer: bad arguments");
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int mpad = M <= 16 ? 16 : 64;
-  const int A = n_heads * 128;
-  if (!chain_phase_ok(H, A, FIN_RESID_NORM) || !chain_phase_ok(2 * I, H, FIN_SWIGLU_IL) || !chain_phase_ok(H, I, FIN_RESID_NORM) ||
-      !chain_phase_ok((n_heads + 2 * n_kv_heads) * 128, H, FIN_QKV_ROPE))
-    return fail("eb200_k_chain_layer: shape not supported by the chain kernel");
-  Scratch sc;
-  float* ws = sc.get<float>(chain_ws_bytes(mpad) / 4, false);
-  int* sync = sc.get<int>(16);
-  if (!ws || !sync) return fail("scratch allocation failed");
-  ChainArgs a;
-  ChainMaps m;
-  memset(&a, 0, sizeof(a));
-  memset(&m, 0, sizeof(m));
-  a.n_phases = n_phases;
-  a.m_rows = M;
-  a.m_idx = -1;
-  a.ws = ws;
-  a.sync = sync;
-  const void* lut = silu_lut(dtype, s);
-  if (!lut) return fail("SiLU table unavailable");
-  auto rows_chunks = [&](int passes) { return std::max(1, std::min(passes, std::max(1, chain_grid()) / M)); };
-  // phase 0: o_proj
-  a.ph[0].N = H; a.ph[0].K = A; a.ph[0].fin = FIN_RESID_NORM; a.ph[0].chunks = 1;
-  a.ph[0].x = x; a.ph[0].ld_x = H; a.ph[0].norm_w = ln2; a.ph[0].xn = xn; a.ph[0].ld_xn = H; a.ph[0].eps = eps;
-  TRY(make_tmap(&m.w[0], dtype, Wo, H, A, 128));
-  TRY(make_tmap(&m.x[0], dtype, attn, 64, A, mpad));
-  if (n_phases > 1) {
-    a.ph[1].N = 2 * I; a.ph[1].K = H; a.ph[1].fin = FIN_SWIGLU_IL; a.ph[1].chunks = rows_chunks((I + 511) / 512);
-    a.ph[1].out = act; a.ph[1].ld_out = I; a.ph[1].silu_lut = lut;
-    TRY(make_tmap(&m.w[1], dtype, Wgu, 2 * I, H, 128));
-    TRY(make_tmap(&m.x[1], dtype, xn, 64, H, mpad));
-  }
-  if (n_phases > 2) {
-    a.ph[2].N = H; a.ph[2].K = I; a.ph[2].fin = FIN_RESID_NORM; a.ph[2].chunks = 1;
-    a.ph[2].x = x; a.ph[2].ld_x = H; a.ph[2].tap = tap; a.ph[2].ld_tap = H; a.ph[2].norm_w = ln1n; a.ph[2].xn = xn; a.ph[2].ld_xn = H; a.ph[2].eps = eps;
-    TRY(make_tmap(&m.w[2], dtype, Wdown, H, I, 128));
-    TRY(make_tmap(&m.x[2], dtype, act, 64, I, mpad));
-  }
-  if (n_phases > 3) {
-    const int NH = n_heads + 2 * n_kv_heads;
-    ChainPhase& q = a.ph[3];
-    q.N = NH * 128; q.K = H; q.fin = FIN_QKV_ROPE; q.chunks = rows_chunks((NH + 7) / 8);
-    q.q_out = q_out; q.k_cache = k_cache; q.v_cache = v_cache; q.kv_cap = kv_cap; q.n_q_heads = n_heads; q.n_kv_heads = n_kv_heads;
-    q.rope_cos = cosp; q.rope_sin = sinp; q.pos_base = DynInt{-1, 0}; q.pos_arr = pos; q.pos_mstride = 0; q.kv_base = DynInt{-1, kv_base};
-    TRY(make_tmap(&m.w[3], dtype, Wqkv, NH * 128, H, 128));
-    TRY(make_tmap(&m.x[3], dtype, xn, 64, H, mpad));
-  }
-  CKL(launch_gemm_chain(dtype, mpad, m, a, s));
-  CK(cudaStreamSynchronize(s));
-  return 0;
-}
-
-// A single GEMM through the chain kernel.  mode 0: stream-K partials + row-wise finish, out = T(X . W^T [+ bias]);
-// mode 1: whole tiles, direct store; mode 2: fused arg-max -> out_idx[M] (int32).  `repeat` launches back to back (exercises
-// the self-resetting phase counters).
+// A single GEMM through the lm_head launch (mega.cu).  mode 1: direct store, out = T(X . W^T [+ bias]); mode 2: fused arg-max ->
+// out_idx[M] (int32).  `repeat` launches back to back (exercises the self-resetting counters).
 extern "C" int eb200_k_chain_gemm(int32_t dtype, int32_t mode, const void* W, const void* X, void* out, const void* bias, int32_t* out_idx,
                                   int32_t M, int32_t N, int32_t K, int32_t repeat, void* stream) {
-  if (M < 1 || M > 64 || mode < 0 || mode > 2 || repeat < 1) return fail("eb200_k_chain_gemm: bad arguments");
+  if (M < 1 || M > 64 || mode < 1 || mode > 2 || repeat < 1) return fail("eb200_k_chain_gemm: bad arguments");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int mpad = M <= 16 ? 16 : 64;
-  const int fin = mode == 0 ? FIN_STORE : (mode == 1 ? FIN_STORE_DIRECT : FIN_ARGMAX);
-  if (!chain_phase_ok(N, K, fin)) return fail("eb200_k_chain_gemm: shape not supported by the chain kernel in this mode");
+  if (!chain_phase_ok(N, K)) return fail("eb200_k_chain_gemm: shape not supported by the chain kernel");
   Scratch sc;
-  float* ws = sc.get<float>(chain_ws_bytes(mpad) / 4, false);
-  int* sync = sc.get<int>(16);
+  int* sync = sc.get<int>(2);
   const int tiles = (N + 127) / 128;
   float* tv = sc.get<float>(static_cast<size_t>(tiles) * 64);
   int* ti = sc.get<int>(static_cast<size_t>(tiles) * 64);
-  if (!ws || !sync || !tv || !ti) return fail("scratch allocation failed");
+  if (!sync || !tv || !ti) return fail("scratch allocation failed");
   ChainArgs a;
   ChainMaps m;
   memset(&a, 0, sizeof(a));
   memset(&m, 0, sizeof(m));
-  a.n_phases = 1;
   a.m_rows = M;
   a.m_idx = -1;
-  a.ws = ws;
   a.sync = sync;
-  ChainPhase& ph = a.ph[0];
-  ph.N = N; ph.K = K; ph.fin = fin;
-  ph.chunks = mode == 0 ? std::max(1, std::min((N + 511) / 512, std::max(1, chain_grid()) / M)) : 1;
+  ChainPhase& ph = a.ph;
+  ph.N = N; ph.K = K; ph.fin = mode == 1 ? FIN_STORE_DIRECT : FIN_ARGMAX;
   ph.out = out; ph.ld_out = N; ph.bias = bias;
   ph.tile_val = tv; ph.tile_idx = ti; ph.out_idx = out_idx;
-  TRY(make_tmap(&m.w[0], dtype, W, N, K, 128));
-  TRY(make_tmap(&m.x[0], dtype, X, 64, K, mpad));
+  TRY(make_tmap(&m.w, dtype, W, N, K, 128));
+  TRY(make_tmap(&m.x, dtype, X, 64, K, mpad));
   for (int r = 0; r < repeat; ++r) CKL(launch_gemm_chain(dtype, mpad, m, a, s));
   CK(cudaStreamSynchronize(s));
   return 0;

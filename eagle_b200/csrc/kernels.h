@@ -145,65 +145,30 @@ const void* silu_lut(int dtype, cudaStream_t s);
 int gemm_stage_count(int mpad, int epi);
 
 // ----------------------------------------------------------------------------------------------
-// persistent GEMM chain (mega.cu): up to 4 dependent skinny GEMMs in ONE launch of one CTA per SM.  Every phase is
-// split stream-K style over all CTAs (equal shares of (n-tile, k-block) units); fp32 partial tiles go to an L2-resident
-// workspace, a per-phase arrival counter replaces the kernel boundary, and the "finish" step (split-K reduction + the
-// reference's epilogue arithmetic + the RMSNorm that feeds the next phase) runs row-wise on the first rows*chunks CTAs.
-// The weight producer never waits for a phase boundary: the next projection's tiles stream into the shared-memory ring
-// while the current one finishes, so HBM stays busy across what used to be 4 launches + 2 RMSNorm launches.
+// lm_head GEMM (mega.cu): ONE launch of one CTA per SM, CTA c owns the whole 128-row weight tiles c, c+G, ...; the epilogue
+// finishes each tile straight from the staged accumulators (no split-K, no partials in global memory).
 // ----------------------------------------------------------------------------------------------
 enum ChainFinish : int {
-  FIN_RESID_NORM = 0,    // x = T(T(acc) + x) in place; optional tap copy; optional xn = w * T(x * rstd)   (o_proj, down_proj)
-  FIN_SWIGLU_IL = 1,     // out = T(T(silu(T(gate))) * T(up)) over the interleaved gate/up matrix           (gate_up)
-  FIN_QKV_ROPE = 2,      // q -> q_out (rope), k -> K cache (rope), v -> V cache                           (qkv)
-  FIN_STORE = 3,         // out = T(acc [+ bias])
-  FIN_ARGMAX = 4,        // whole tiles per CTA, per-tile (max, first index) from the staged tile, merged per row (verify lm_head)
-  FIN_STORE_DIRECT = 5,  // whole tiles per CTA, out = T(acc [+ bias]) from the staged tile                (lm_head, sampling path)
+  FIN_ARGMAX,        // per-tile (max, first index) from the staged tile, merged per row (verify lm_head)
+  FIN_STORE_DIRECT,  // out = T(acc [+ bias]) from the staged tile                  (lm_head, sampling path)
 };
-constexpr int kChainMaxPhases = 4;
 struct ChainPhase {
-  int N, K;      // weight rows (interleaved rows for FIN_SWIGLU_IL), reduction length
+  int N, K;      // weight rows, reduction length
   int fin;       // ChainFinish
-  int chunks;    // finish work items per activation row (column ranges handled by different CTAs); 1 for FIN_RESID_NORM
-  // FIN_RESID_NORM
-  void* x;             // output (and, when res == nullptr, the residual input: in place)
-  long ld_x;
-  const void* res;     // optional separate residual input (the draft head keeps d_h / d_h2 / d_out apart)
-  long ld_res;
-  void* tap;     // optional second copy of the new x row (EAGLE-3 feature tap: hidden state entering layers 2, L/2, L-3)
-  long ld_tap;
-  const void* norm_w;  // optional RMSNorm weight; output -> xn (the next phase's X operand)
-  void* xn;
-  long ld_xn;
-  float eps;
-  // FIN_SWIGLU_IL / FIN_STORE / FIN_STORE_DIRECT
+  // FIN_STORE_DIRECT
   void* out;
   long ld_out;
   const void* bias;
-  const void* silu_lut;
-  // FIN_QKV_ROPE (same meaning as GemmParams)
-  void* q_out;
-  void* k_cache;
-  void* v_cache;
-  long kv_cap;
-  int n_q_heads, n_kv_heads;
-  const void* rope_cos;
-  const void* rope_sin;
-  DynInt pos_base;
-  const int* pos_arr;
-  int pos_mstride;
-  DynInt kv_base;
   // FIN_ARGMAX
   float* tile_val;  // [n_tiles][64]
   int* tile_idx;    // [n_tiles][64]
   int* out_idx;     // [rows]
   int idx_offset;   // tensor parallel: first vocabulary row of this rank's lm_head shard
 };
-// Tensor parallelism inside the chain kernel: every rank's "window" (one cudaMalloc block, opened on the peers through CUDA
-// IPC) holds the replicated activations (x, xn, feature taps), a per-source inbox for fp32 partial rows and the flags.  A
-// row-parallel projection (o_proj, down_proj) then finishes in the SAME launch: each rank reduces its own split-K partials
-// of row m and pushes the fp32 row over NVLink into the inbox of the row's owner (m % tp); the owner adds the tp rows in rank
-// order, applies the residual + RMSNorm and pushes the new x / xn rows back to every rank.  No NCCL call, no extra kernel.
+// Tensor parallelism over NVLink peer memory: every rank's "window" (one cudaMalloc block, opened on the peers through CUDA
+// IPC) holds the replicated activations (x, xn, feature taps), a per-source inbox for fp32 partial rows, the row flags and
+// the lm_head's arg-max exchange.  The row-parallel projections (o_proj, down_proj) finish in tp_fused.cu behind the
+// per-projection GEMMs; the vocabulary-parallel arg-max of the lm_head exchanges its (value, index) pairs in the chain launch.
 constexpr int kMaxTp = 8;
 struct ChainTP {
   int size, rank;
@@ -211,10 +176,9 @@ struct ChainTP {
   long inbox_off;           // float [tp][64][ld_inbox]
   long ld_inbox;
   long flag_off;            // int [tp][64]: epoch of the last row pushed by (src, m)
-  long ready_off;           // int: rows of finished TP phases received (monotonic)
+  long ready_off;           // 1 KB block, ints [64, 128): row flags of the two-shot exchange (tp_fused.cu)
   long am_off;              // arg-max exchange: float2-like {val, idx} [tp][64], then int flags [tp][64]
-  int* epoch;               // local: TP phases executed so far (monotonic; identical on every rank)
-  int* ready_base;          // local: value of the ready counter when the running launch started
+  int* epoch;               // local: exchanges executed so far (monotonic; identical on every rank)
 };
 // standalone form of the same exchange behind the per-projection GEMMs (tp_fused.cu): all-reduce + residual + RMSNorm in one launch
 struct TpResidParams {
@@ -236,28 +200,21 @@ struct TpResidParams {
 int launch_tp_resid_norm(int dtype, const TpResidParams& p, int rows, cudaStream_t s);
 struct ChainArgs {
   ChainTP tp;
-  int n_phases;
   int m_rows, m_idx;  // valid activation rows = min(m_rows, st[m_idx]) (m_idx < 0: m_rows)
   const int* st;
-  float* ws;          // >= chain_ws_bytes(mpad)
-  int* sync;          // >= 16 zeroed ints, owned by this stream (self-resetting)
+  int* sync;          // >= 2 zeroed ints, owned by this stream (self-resetting)
   // optional in-kernel timing (works inside a replayed CUDA graph, no profiler): [0] += ns from "dependencies resolved" on CTA 0
   // to the exit of the last CTA, [1] += 1 per launch, [2] scratch (start stamp of the running launch)
   unsigned long long* timing;
-  unsigned long long* trace;  // optional [CTAs][32] %globaltimer stamps (EB200_CHAIN_TRACE; see tools/chain_trace.py)
-  int w_ahead;        // weight tiles (per CTA) the producer may load for phase p+1 before finish(p) has completed (<0: no limit)
-  int l2_window;      // weight tiles (16 KB each, per CTA) the producer may prefetch into L2 beyond the shared-memory ring
-  ChainPhase ph[kChainMaxPhases];
+  ChainPhase ph;
 };
 struct ChainMaps {
-  CUtensorMap w[kChainMaxPhases];  // weights [N][K], box 128 x 64
-  CUtensorMap x[kChainMaxPhases];  // activations [64][K], box mpad x 64
+  CUtensorMap w;  // weights [N][K], box 128 x 64
+  CUtensorMap x;  // activations [64][K], box mpad x 64
 };
 int launch_gemm_chain(int dtype, int mpad, const ChainMaps& maps, const ChainArgs& args, cudaStream_t s);
-size_t chain_ws_bytes(int mpad);
-int chain_grid();  // CTAs of a chain launch on the current device (= its SM count)
-// can this (N, K, finish) run as a chain phase on the current device?  (slot count, 32-bit unit arithmetic, alignment)
-bool chain_phase_ok(int N, int K, int fin);
+// can an [N, K] weight run through the lm_head launch on the current device?  (TMA row stride, device attributes)
+bool chain_phase_ok(int N, int K);
 
 // ----------------------------------------------------------------------------------------------
 // elementwise / reduction kernels (misc.cu)

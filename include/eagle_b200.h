@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define EB200_ABI_VERSION 4
+#define EB200_ABI_VERSION 5
 
 enum { EB200_BF16 = 0, EB200_FP16 = 1 };
 enum { EB200_DT_BF16 = 0, EB200_DT_FP16 = 1, EB200_DT_FP32 = 2, EB200_DT_INT64 = 3, EB200_DT_BOOL = 4, EB200_DT_INT8 = 5, EB200_DT_UINT8 = 6,
@@ -61,11 +61,11 @@ typedef struct eb200_config {
 
 #define EB200_FLAG_SIMT_GEMM 1   /* bring-up only: route GEMMs through the plain-FMA kernel */
 #define EB200_FLAG_NO_GRAPH 2    /* launch kernels directly instead of replaying the captured cycle graph */
-#define EB200_FLAG_NO_CHAIN 4    /* one kernel per projection / RMSNorm instead of the persistent per-layer chain launches */
+#define EB200_FLAG_NO_CHAIN 4    /* target lm_head as a GEMM launch + vocab_argmax instead of the fused arg-max launch */
 /* The q/k/v/o/gate/up/down projections of every TARGET decoder layer are stored as int8 plus one fp32 scale per row
  * (bitsandbytes' 8-bit weight format) and multiplied by a W8A16 GEMM that computes exactly what the model-dtype GEMM computes on
  * W' = dtype((q * SCB) * 7.874015718698502e-3).  lm_head, embeddings, norms and the draft head stay in the model dtype.
- * Single GPU, default GEMM path only: eb200_finalize refuses tp_size > 1, EB200_FLAG_SIMT_GEMM and EB200_CHAIN=1. */
+ * Single GPU, default GEMM path only: eb200_finalize refuses tp_size > 1 and EB200_FLAG_SIMT_GEMM. */
 #define EB200_FLAG_TARGET_INT8 8
 /* The same projections stored as bitsandbytes 4-bit codes (NF4 or FP4 table, blocksize 64: one fp32 absmax per 64 consecutive
  * elements of a row) and multiplied by a W4A16 GEMM that computes exactly what the model-dtype GEMM computes on
@@ -130,8 +130,8 @@ int eb200_tp_shard(const char* name, int64_t rows, int64_t cols, int32_t tp_rank
 int eb200_tp_init(eb200_engine* e, const void* id128);
 /* NVLink peer windows (optional, after eb200_tp_init and before eb200_finalize): each rank exports a 64-byte CUDA IPC handle, the
  * launcher all-gathers them and every rank opens the others'.  With the peers open, the row-parallel projections are reduced
- * inside the per-layer chain launch over peer memory (no NCCL call on the decode path).  eb200_tp_open_peers fails (and the engine
- * keeps the NCCL path) when the GPUs have no peer access. */
+ * over peer memory by one kernel behind each of them, and the lm_head's arg-max is exchanged through the same windows (no NCCL
+ * call on the decode path).  eb200_tp_open_peers fails (and the engine keeps the NCCL path) when the GPUs have no peer access. */
 int eb200_tp_ipc_handle(eb200_engine* e, void* out64);
 int eb200_tp_open_peers(eb200_engine* e, const void* handles, int32_t n);
 
@@ -205,7 +205,7 @@ typedef struct eb200_stats {
   uint64_t gemm_launches;
   double attn_ms, other_ms;
   double verify_gemm_ms, verify_gemm_bytes;  /* the target verify pass' share */
-  /* persistent chain kernel, measured INSIDE the kernel with %globaltimer (valid under graph replay, no profiler): time from
+  /* lm_head launch (mega.cu), measured INSIDE the kernel with %globaltimer (valid under graph replay, no profiler): time from
    * "dependencies resolved" on CTA 0 to the exit of the last CTA, summed over launches; algorithmic weight bytes of those launches */
   double chain_ms, chain_bytes;
   uint64_t chain_launches;
@@ -237,18 +237,13 @@ int eb200_k_gemm_fp8(int32_t dtype, int32_t epilogue, const void* Wq, const void
                      const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
 int eb200_k_gemm_w4(int32_t dtype, int32_t quant_type, int32_t epilogue, const void* Wq, const void* absmax, const void* X, void* out,
                     const void* res, const void* bias, int32_t M, int32_t N, int32_t K, int32_t splitk, void* stream);
+/* the lm_head launch (mega.cu, whole 128-row weight tiles per CTA) as a single GEMM: mode 1 stores out = T(X . W^T [+ bias]),
+ * mode 2 writes the fused arg-max of every row to out_idx (int32); any other mode is refused.  `repeat` launches back to back. */
+int eb200_k_chain_gemm(int32_t dtype, int32_t mode, const void* W, const void* X, void* out, const void* bias, int32_t* out_idx,
+                       int32_t M, int32_t N, int32_t K, int32_t repeat, void* stream);
 /* micro-benchmark of the skinny GEMM: `iters` back-to-back launches cycling over `n_weights` distinct [N,K] weight
  * matrices (so the stream is HBM-, not L2-resident), timed with CUDA events; optionally replayed from a CUDA graph.
  * epilogue: 0 store, 1 residual, 2 swiglu.  Returns the average microseconds per launch. */
-/* persistent per-layer chain kernel (mega.cu) on caller tensors: the o_proj -> gate/up -> down_proj -> next qkv segment
- * that replaces modeling_llama_kv.py:801-863 per decoder layer (n_phases 1..4 stops early), and a single GEMM in its three
- * modes (0 stream-K + finish store, 1 direct store, 2 fused arg-max).  All pointers are device pointers. */
-int eb200_k_chain_layer(int32_t dtype, int32_t M, int32_t H, int32_t I, int32_t n_heads, int32_t n_kv_heads, int32_t n_phases,
-                        const void* Wo, const void* Wgu, const void* Wdown, const void* Wqkv, const void* ln2, const void* ln1n,
-                        const void* attn, void* x, void* xn, void* act, void* tap, void* q_out, void* k_cache, void* v_cache,
-                        int64_t kv_cap, const void* cos, const void* sin, const int32_t* pos, int32_t kv_base, float eps, void* stream);
-int eb200_k_chain_gemm(int32_t dtype, int32_t mode, const void* W, const void* X, void* out, const void* bias, int32_t* out_idx,
-                       int32_t M, int32_t N, int32_t K, int32_t repeat, void* stream);
 int eb200_k_gemm_bench(int32_t dtype, int32_t epilogue, int32_t M, int32_t N, int32_t K, int32_t splitk, int32_t n_weights,
                        int32_t iters, int32_t use_graph, double* us_per_launch);
 int eb200_k_rmsnorm(int32_t dtype, const void* x, const void* w, void* y, int32_t rows, int32_t H, float eps, void* stream);

@@ -239,15 +239,11 @@ def test_from_pretrained_fp8(tmp_path):
         assert got[0].cpu().tolist() == want[0].cpu().tolist() and got[1:] == want[1:], kw
 
 
-def test_engine_refusals_with_fp8_weights(monkeypatch):
+def test_engine_refusals_with_fp8_weights():
     from eagle_b200 import EaModel, _lib
     tcfg, tW, hcfg, hW, eagle3, dtype, tree = fixture_models("e3_corr_bf16")
     t8, _ = split_weights(tW, dtype)
     common = dict(use_eagle3=eagle3, torch_dtype=dtype, max_length=512, **tree)
-    monkeypatch.setenv("EB200_CHAIN", "1")
-    with pytest.raises(_lib.EngineError, match="EB200_CHAIN=1"):
-        EaModel.from_state_dicts(tcfg, t8, hcfg, hW, quantization_config=FP8, **common)
-    monkeypatch.delenv("EB200_CHAIN")
     with pytest.raises(_lib.EngineError, match="EB200_FLAG_SIMT_GEMM"):
         EaModel.from_state_dicts(tcfg, t8, hcfg, hW, quantization_config=FP8, flags=_lib.FLAG_SIMT_GEMM, **common)
     for other in (_lib.FLAG_TARGET_INT8, _lib.FLAG_TARGET_NF4, _lib.FLAG_TARGET_FP4):

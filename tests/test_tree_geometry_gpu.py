@@ -339,17 +339,6 @@ def test_int8_twin_at_the_default_geometry():
         assert same(ca[c], cb[c]), f"cycle {c - 1}: int8 engine and its model-dtype twin differ"
 
 
-@pytest.mark.parametrize("env", ["EB200_CHAIN", "EB200_CHAIN_DRAFT"])
-def test_chain_launch_paths_at_the_default_geometry(env, monkeypatch):
-    """The persistent chain launches (read from the environment when the engine is finalized) take the same tree masks."""
-    monkeypatch.setenv(env, "1")
-    base = "e3_corr_bf16"
-    w = weights(base)
-    m = engine(w, DEFAULT)
-    monkeypatch.delenv(env)
-    compare_cycles(m, oracle(w, DEFAULT), prompt_of(base, w), DEFAULT, f"{env}=1 {tid(DEFAULT)}")
-
-
 def test_static_tree_next_to_a_wide_dynamic_engine():
     """A fixed tree is untouched by the dynamic-tree geometry of another engine in the same process."""
     from eagle_b200 import static_trees

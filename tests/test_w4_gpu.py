@@ -253,16 +253,12 @@ def test_from_pretrained_4bit(tmp_path):
         assert got[0].cpu().tolist() == want[0].cpu().tolist() and got[1:] == want[1:], d
 
 
-def test_engine_refusals_with_4bit_weights(monkeypatch):
+def test_engine_refusals_with_4bit_weights():
     from eagle_b200 import EaModel, _lib
     tcfg, tW, hcfg, hW, eagle3, dtype, tree = fixture_models("e3_corr_bf16")
     t4, _ = split_weights(tW, dtype, "nf4")
     t8 = {k: quant.quantize_int8_rowwise(v)[0] for k, v in tW.items() if k.endswith("down_proj.weight")}
     common = dict(use_eagle3=eagle3, torch_dtype=dtype, max_length=512, **tree)
-    monkeypatch.setenv("EB200_CHAIN", "1")
-    with pytest.raises(_lib.EngineError, match="EB200_CHAIN=1"):
-        EaModel.from_state_dicts(tcfg, t4, hcfg, hW, quantization_config=qc("nf4"), **common)
-    monkeypatch.delenv("EB200_CHAIN")
     with pytest.raises(_lib.EngineError, match="EB200_FLAG_SIMT_GEMM"):
         EaModel.from_state_dicts(tcfg, t4, hcfg, hW, quantization_config=qc("nf4"), flags=_lib.FLAG_SIMT_GEMM, **common)
     with pytest.raises(_lib.EngineError, match="exclude each other"):
